@@ -1,5 +1,5 @@
 /*
- * pd_b200.h — C ABI of libpd_b200.so: hand-written sm_100a kernels behind the PyDreamer
+ * pd_b200.h — C ABI of libpd_b200.so: hand-written sm_90a kernels behind the PyDreamer
  * world-model training step + imagination rollout (BASELINE.json north_star; SURVEY.md §8).
  *
  * The reference (jurgisp/pydreamer) has no FFI: its boundary is the Python class
@@ -36,12 +36,15 @@ typedef struct pd_handle pd_handle;
 #define PD_ACT_NONE 0
 #define PD_ACT_ELU 1
 
-#define PD_GEMM_TCGEN05 0 /* tcgen05.mma kind::tf32 + TMA + TMEM (default, the product path) */
+#define PD_GEMM_TC 0      /* TMA-fed tensor-core (mma.sync tf32 / fp16) kernel (default, the product path) */
 #define PD_GEMM_SIMT 1    /* plain fp32 CUDA-core tile kernel: validation arm for the tests  */
 #define PD_GEMM_C_ZEROED 1 /* pd_gemm flags bit */
 #define PD_GEMM_C_F16 2    /* pd_gemm flags bit: C is an fp16 matrix (ldc in halfs); not with accumulate */
 
 /* ---- lifetime ---------------------------------------------------------------------------- */
+/* A handle allocates 8 scratch areas of 16 MB on its device for the fixed-order gradient reductions, one per stream it
+ * launches on, bound to a stream at its first reduction and kept for the handle's lifetime.  Reductions on a ninth stream
+ * fail with PD_ERR_UNSUPPORTED: use one handle per set of at most eight streams. */
 int pd_create(int device_ordinal, pd_handle** out);
 void pd_destroy(pd_handle* h);
 const char* pd_last_error(const pd_handle* h);
@@ -56,13 +59,13 @@ int pd_set_round_operands(pd_handle* h, int on);
 /* C[M,N] (=|+=) sum_k A(m,k) * B(n,k)  [+ bias[n]] [+ R[m / r_div, n]] -> act -> (tf32 round)
  *   a_mn = 0: A stored [M][K] (K contiguous, row stride lda); a_mn = 1: A stored [K][M] (M contiguous).
  *   b_mn = 0: B stored [N][K] (nn.Linear weight layout);      b_mn = 1: B stored [K][N].
- *   accumulate = 1: atomically adds into C (split-K over all SMs; bias/R/act must be off).
+ *   accumulate = 1: adds into C (split-K partials are summed in a fixed order; bias/R/act must be off).
  * Replaces every nn.Linear / nn.GRUCell matmul and the conv/deconv contractions:
  * common.py:47-55, rssm.py:103-116,138-146, rnn.py:60-67, encoders.py:80-90, decoders.py:128-155.
- * flags: PD_GEMM_C_ZEROED = the caller has already cleared C (skinny-M launches that split K skip their own clear);
+ * flags: PD_GEMM_C_ZEROED = the caller has already cleared C (accepted; the kernel never needs to clear C itself);
  *        PD_GEMM_C_F16 = C points to an fp16 matrix (the deconvolution column matrices of the decoder forward: they are
  *        written once and read once, in fp16 they cost half the HBM traffic; decoders.py:149-155).
- * TMA constraints (tcgen05 impl): lda/ldb multiples of 4 elements, base pointers 16-byte aligned. */
+ * TMA constraints (tensor-core impl): lda/ldb multiples of 4 elements, base pointers 16-byte aligned. */
 int pd_gemm(pd_handle* h, int M, int N, int K,
             const float* A, long lda, int a_mn,
             const float* B, long ldb, int b_mn,
@@ -70,7 +73,7 @@ int pd_gemm(pd_handle* h, int M, int N, int K,
             const float* bias, const float* R, long ldr, int r_div,
             int act, int round_out, int accumulate, int flags, void* stream);
 
-/* Forward-only contraction with fp16 operands (tcgen05 kind::f16, fp32 accumulate / output): same 10-bit mantissa as
+/* Forward-only contraction with fp16 operands (mma.sync f16, fp32 accumulate / output): same 10-bit mantissa as
  * TF32 at twice the tensor rate and half the operand bytes.  Used where no gradient flows through the GEMM (the
  * imagination rollout and the heads evaluated on dreamed features, dreamer.py:188-216, a2c.py:88,112).
  * A: [M][K] fp16, B: [N][K] fp16 (both K-major, ld % 8 == 0), C fp32. */
@@ -241,12 +244,13 @@ int pd_bias_act_bwd(pd_handle* h, long M, int N, float* dy, long lddy, const flo
                     int act, float* db, void* stream);
 /* The ELU backward + bias gradient of the layer BELOW fused into the kernel that produces that layer's output gradient
  * (instead of a separate pd_bias_act_bwd pass over the gradient image; PD_B200_FUSE_ACTBWD=0 composes the two launches):
- *   pd_gemm_actbwd:      C = (A B^T) .* elu'(dact), dbias[n] += sum_m C[m, n]      (Linear / explicit-column deconv dX;
+ *   pd_gemm_actbwd:      C = (A B^T) .* elu'(dact) in the GEMM epilogue, then dbias[n] += sum_m C[m, n] (Linear / explicit-column deconv dX;
  *                        decoders.py:128-155 backward, autograd of nn.ELU + bias)
  *   pd_conv_gemm_actbwd: the same for pd_conv_gemm mode 1 (ConvTranspose2d input gradient gathered by TMA im2col)
  *   pd_col2im_actbwd:    out = fold(col) .* elu'(dact), dbias[c] += sum over pixels  (Conv2d input gradient; encoders.py:80-90
  *                        backward); out / dact contiguous NHWC [NB, Hout, Wout, Cc], Hout >= 2(Hin-1)+k (rows a stride-2 conv never read get 0)
- * dact is the saved forward output of the layer below (ELU derivative from the output: y > 0 ? 1 : y + 1). */
+ * dact is the saved forward output of the layer below (ELU derivative from the output: y > 0 ? 1 : y + 1).
+ * Every bias / LayerNorm gradient of this ABI is summed in a fixed order: the same inputs give bit-identical results. */
 int pd_gemm_actbwd(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_mn, const float* B, long ldb, int b_mn,
                    float* C, long ldc, const float* dact, long lddact, float* dbias, void* stream);
 int pd_conv_gemm_actbwd(pd_handle* h, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo, int o_mn,

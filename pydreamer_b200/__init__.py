@@ -1,4 +1,4 @@
-"""pydreamer_b200 — B200-native (sm_100a) drop-in for the hot path of jurgisp/pydreamer:
+"""pydreamer_b200 — H100-native (sm_90a) drop-in for the hot path of jurgisp/pydreamer:
 `Dreamer.training_step` (world-model step + imagination rollout + actor-critic losses), its gradients,
 grad-clip and AdamW — hand-written CUDA kernels behind the reference's own module API."""
 from .config import make_conf  # noqa: F401

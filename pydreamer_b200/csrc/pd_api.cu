@@ -2,17 +2,33 @@
 #include "pd_common.cuh"
 #include <stdlib.h>
 
-int pd_gemm_tcgen05_launch(pd_handle* h, int M, int N, int K, const void* A, long lda, int a_mn, const void* B,
-                           long ldb, int b_mn, const PdEpilogue& epi, cudaStream_t stream, int f16);
+int pd_gemm_tc_launch(pd_handle* h, int M, int N, int K, const void* A, long lda, int a_mn, const void* B,
+                      long ldb, int b_mn, const PdEpilogue& epi, cudaStream_t stream, int f16);
 int pd_gemm_simt_launch(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_mn, const float* B,
                         long ldb, int b_mn, const PdEpilogue& epi, cudaStream_t stream);
 
 int pd_conv_gemm_launch(pd_handle* h, int mode, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo,
                         int o_mn, int ODIM, const PdEpilogue& epi, cudaStream_t stream);
 
+int pd_scratch(pd_handle* h, cudaStream_t stream, long nfloats, int ngroups, float** ws, unsigned** tickets) {
+    PD_REQUIRE(h, nfloats <= PD_SCRATCH_FLOATS && ngroups <= PD_SCRATCH_TICKETS,
+               "reduction needs %ld partials / %d groups, the scratch area holds %ld / %d", nfloats, ngroups, PD_SCRATCH_FLOATS,
+               PD_SCRATCH_TICKETS);
+    for (int i = 0; i < PD_SCRATCH_SLOTS; ++i) {
+        PdScratch& sc = h->scratch[i];
+        if (!sc.used) { sc.used = 1; sc.stream = stream; }
+        if (sc.stream == stream) {
+            *ws = sc.ws;
+            *tickets = sc.tickets;
+            return PD_OK;
+        }
+    }
+    PD_FAIL(h, PD_ERR_UNSUPPORTED, "more than %d streams on one handle", PD_SCRATCH_SLOTS);
+}
+
 extern "C" {
 
-const char* pd_version(void) { return "pd_b200 0.1 (sm_100a; tcgen05 tf32 + TMA)"; }
+const char* pd_version(void) { return "pd_b200 0.1 (sm_90a; TMA + mbarrier pipelines, mma.sync tf32 / fp16)"; }
 
 int pd_create(int device_ordinal, pd_handle** out) {
     if (!out) return PD_ERR_ARG;
@@ -21,37 +37,30 @@ int pd_create(int device_ordinal, pd_handle** out) {
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || device_ordinal < 0 || device_ordinal >= ndev) return PD_ERR_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device_ordinal) != cudaSuccess) return PD_ERR_DEVICE;
-    if (prop.major != 10) return PD_ERR_UNSUPPORTED;   // sm_100a only: no fallback paths
+    if (prop.major != 9) return PD_ERR_UNSUPPORTED;    // sm_90a only: no fallback paths
     pd_handle* h = (pd_handle*)calloc(1, sizeof(pd_handle));
     if (!h) return PD_ERR_DEVICE;
     h->device = device_ordinal;
     h->num_sms = prop.multiProcessorCount;
     h->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
-    h->gemm_impl = PD_GEMM_TCGEN05;
+    h->gemm_impl = PD_GEMM_TC;
     h->round_ops = 1;
-    h->gemm_2cta = 1;
-    if (const char* e2 = getenv("PD_GEMM_2CTA")) h->gemm_2cta = atoi(e2);
-    h->gemm_mn3 = 1;
-    h->gemm_conv_k64 = 1;
-    h->gemm_conv_2cta = 1;
-    h->gemm_conv_m2 = 1;
-    h->gemm_plain_m2 = 0;
-    if (const char* e11 = getenv("PD_GEMM_PLAIN_M2")) h->gemm_plain_m2 = atoi(e11);
-    h->gemm_2cta_k2 = 0;
-    if (const char* e10 = getenv("PD_GEMM_2CTA_K2")) h->gemm_2cta_k2 = atoi(e10);
-    if (const char* e9 = getenv("PD_GEMM_CONV_M2")) h->gemm_conv_m2 = atoi(e9);
-    if (const char* e8 = getenv("PD_GEMM_CONV_2CTA")) h->gemm_conv_2cta = atoi(e8);
-    h->gemm_2cta_min_m = 384;
     h->fuse_actbwd = 1;
     if (const char* e7 = getenv("PD_B200_FUSE_ACTBWD")) h->fuse_actbwd = atoi(e7);
-    if (const char* e6 = getenv("PD_GEMM_2CTA_MINM")) h->gemm_2cta_min_m = atoi(e6);
-    if (const char* e4 = getenv("PD_GEMM_CONV_K64")) h->gemm_conv_k64 = atoi(e4);
-    if (const char* e3 = getenv("PD_GEMM_MN3")) h->gemm_mn3 = atoi(e3);
     cudaSetDevice(device_ordinal);
+    for (int i = 0; i < PD_SCRATCH_SLOTS; ++i) {
+        PdScratch& sc = h->scratch[i];
+        if (cudaMalloc(&sc.ws, PD_SCRATCH_FLOATS * sizeof(float)) != cudaSuccess ||
+            cudaMalloc(&sc.tickets, PD_SCRATCH_TICKETS * sizeof(unsigned)) != cudaSuccess ||
+            cudaMemset(sc.tickets, 0, PD_SCRATCH_TICKETS * sizeof(unsigned)) != cudaSuccess) {
+            pd_destroy(h);
+            return PD_ERR_DEVICE;
+        }
+    }
     cudaDriverEntryPointQueryResult qres;
     void* fn = nullptr;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) {
-        free(h);
+        pd_destroy(h);
         return PD_ERR_DEVICE;
     }
     h->encode_tiled = fn;
@@ -59,13 +68,21 @@ int pd_create(int device_ordinal, pd_handle** out) {
     return PD_OK;
 }
 
-void pd_destroy(pd_handle* h) { free(h); }
+void pd_destroy(pd_handle* h) {
+    if (!h) return;
+    PdDeviceGuard guard(h);
+    for (int i = 0; i < PD_SCRATCH_SLOTS; ++i) {
+        cudaFree(h->scratch[i].ws);
+        cudaFree(h->scratch[i].tickets);
+    }
+    free(h);
+}
 const char* pd_last_error(const pd_handle* h) { return h ? h->err : "null handle"; }
 long pd_launch_count(const pd_handle* h) { return h ? h->launches : 0; }
 
 int pd_set_gemm_impl(pd_handle* h, int impl) {
     if (!h) return PD_ERR_ARG;
-    PD_REQUIRE(h, impl == PD_GEMM_TCGEN05 || impl == PD_GEMM_SIMT, "unknown gemm impl %d", impl);
+    PD_REQUIRE(h, impl == PD_GEMM_TC || impl == PD_GEMM_SIMT, "unknown gemm impl %d", impl);
     h->gemm_impl = impl;
     return PD_OK;
 }
@@ -85,9 +102,9 @@ int pd_gemm(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_m
     PD_REQUIRE(h, !(accumulate && (bias || R || act)), "pd_gemm: accumulate excludes bias/residual/act");
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
-    e.act = act; e.round_out = round_out; e.accumulate = accumulate; e.c_zeroed = (flags & PD_GEMM_C_ZEROED) ? 1 : 0;
+    e.act = act; e.round_out = round_out; e.accumulate = accumulate;
     e.c_f16 = (flags & PD_GEMM_C_F16) ? 1 : 0;
-    e.dact = nullptr; e.lddact = 0; e.dbias = nullptr;
+    e.dact = nullptr; e.lddact = 0;
     PD_REQUIRE(h, !(e.c_f16 && accumulate), "pd_gemm: an fp16 output cannot accumulate");
     // Skinny / unaligned contractions (scalar heads N=1, action inputs K=18, ...) cannot be described
     // by a TMA tensor map (16-byte strides) and have no tensor-core work to speak of: CUDA cores.
@@ -96,7 +113,7 @@ int pd_gemm(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_m
                         (!e.c_f16 || ((ldc % 8 == 0) && !R && !round_out && ((((uintptr_t)C) & 15) == 0)));
     if (h->gemm_impl == PD_GEMM_SIMT || !tma_ok)
         return pd_gemm_simt_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream);
-    return pd_gemm_tcgen05_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
+    return pd_gemm_tc_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
 }
 
 int pd_conv_gemm(pd_handle* h, int mode, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo, int o_mn,
@@ -106,8 +123,8 @@ int pd_conv_gemm(pd_handle* h, int mode, int NB, int H, int W, int C, int k, con
     PD_REQUIRE(h, (mode == 1) == (accumulate == 0), "pd_conv_gemm: mode 1 stores, modes 2/3 accumulate");
     PdEpilogue e;
     e.C = Cmat; e.ldc = ldc; e.bias = bias; e.R = nullptr; e.ldr = 0; e.r_div = 1;
-    e.act = act; e.round_out = round_out; e.accumulate = accumulate; e.c_zeroed = 0; e.c_f16 = 0;
-    e.dact = nullptr; e.lddact = 0; e.dbias = nullptr;
+    e.act = act; e.round_out = round_out; e.accumulate = accumulate; e.c_f16 = 0;
+    e.dact = nullptr; e.lddact = 0;
     return pd_conv_gemm_launch(h, mode, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
 }
 
@@ -118,14 +135,14 @@ int pd_gemm_f16(pd_handle* h, int M, int N, int K, const void* A, long lda, cons
     PD_REQUIRE(h, A && B && C, "pd_gemm_f16: null operand");
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
-    e.act = act; e.round_out = round_out; e.accumulate = 0; e.c_zeroed = 0; e.c_f16 = 0;
-    e.dact = nullptr; e.lddact = 0; e.dbias = nullptr;
-    return pd_gemm_tcgen05_launch(h, M, N, K, A, lda, 0, B, ldb, 0, e, (cudaStream_t)stream, 1);
+    e.act = act; e.round_out = round_out; e.accumulate = 0; e.c_f16 = 0;
+    e.dact = nullptr; e.lddact = 0;
+    return pd_gemm_tc_launch(h, M, N, K, A, lda, 0, B, ldb, 0, e, (cudaStream_t)stream, 1);
 }
 
-// Input gradient of a layer followed by the backward of the ELU that preceded it in the forward pass, in one launch:
-//   C = (A B^T) * elu'(dact) (tf32-rounded if round_out), dbias[n] += sum_m C[m, n].
-// Falls back to GEMM + pd_bias_act_bwd where the tcgen05 epilogue cannot take it (C not TMA-addressable, SIMT arm).
+// Input gradient of a layer followed by the backward of the ELU that preceded it in the forward pass:
+//   C = (A B^T) * elu'(dact) (tf32-rounded if round_out) in the GEMM's epilogue, then dbias[n] += sum_m C[m, n] (pd_colsum).
+// Falls back to GEMM + pd_bias_act_bwd where the tensor-core epilogue cannot take it (C not TMA-addressable, SIMT arm).
 int pd_gemm_actbwd(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_mn, const float* B, long ldb, int b_mn,
                    float* C, long ldc, const float* dact, long lddact, float* dbias, void* stream) {
     if (!h) return PD_ERR_ARG;
@@ -139,9 +156,11 @@ int pd_gemm_actbwd(pd_handle* h, int M, int N, int K, const float* A, long lda, 
     }
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = nullptr; e.R = nullptr; e.ldr = 0; e.r_div = 1;
-    e.act = PD_ACT_NONE; e.round_out = h->round_ops; e.accumulate = 0; e.c_zeroed = 0; e.c_f16 = 0;
-    e.dact = dact; e.lddact = lddact; e.dbias = dbias;
-    return pd_gemm_tcgen05_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
+    e.act = PD_ACT_NONE; e.round_out = h->round_ops; e.accumulate = 0; e.c_f16 = 0;
+    e.dact = dact; e.lddact = lddact;
+    int rc = pd_gemm_tc_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
+    if (rc || !dbias) return rc;
+    return pd_colsum(h, M, N, C, ldc, dbias, stream);
 }
 
 // The same for the implicit-GEMM convolution form 1 (ConvTranspose2d input gradient, decoders.py:149-155 backward).
@@ -151,16 +170,19 @@ int pd_conv_gemm_actbwd(pd_handle* h, int NB, int H, int W, int C, int k, const 
     PD_REQUIRE(h, X && O && Cmat && dact, "pd_conv_gemm_actbwd: bad arguments");
     PdEpilogue e;
     e.C = Cmat; e.ldc = ldc; e.bias = nullptr; e.R = nullptr; e.ldr = 0; e.r_div = 1;
-    e.act = PD_ACT_NONE; e.round_out = 0; e.accumulate = 0; e.c_zeroed = 0; e.c_f16 = 0;
-    e.dact = nullptr; e.lddact = 0; e.dbias = nullptr;
+    e.act = PD_ACT_NONE; e.round_out = 0; e.accumulate = 0; e.c_f16 = 0;
+    e.dact = nullptr; e.lddact = 0;
     if (!h->fuse_actbwd) {
         int rc = pd_conv_gemm_launch(h, 1, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
         if (rc) return rc;
         const int P = (H - k) / 2 + 1, Q = (W - k) / 2 + 1;
         return pd_bias_act_bwd(h, (long)NB * P * Q, odim, Cmat, ldc, dact, lddact, PD_ACT_ELU, dbias, stream);
     }
-    e.round_out = h->round_ops; e.dact = dact; e.lddact = lddact; e.dbias = dbias;
-    return pd_conv_gemm_launch(h, 1, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
+    e.round_out = h->round_ops; e.dact = dact; e.lddact = lddact;
+    int rc = pd_conv_gemm_launch(h, 1, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
+    if (rc || !dbias) return rc;
+    const int P = (H - k) / 2 + 1, Q = (W - k) / 2 + 1;
+    return pd_colsum(h, (long)NB * P * Q, odim, Cmat, ldc, dbias, stream);
 }
 
 }  // extern "C"

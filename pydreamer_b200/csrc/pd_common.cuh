@@ -1,4 +1,4 @@
-// pydreamer_b200 — shared device/host helpers for the sm_100a kernels.
+// pydreamer_b200 — shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -10,34 +10,47 @@
 #include "../../include/pd_b200.h"
 
 // ---------------------------------------------------------------------------
-// Handle: host-side state only (no device allocations, see include/pd_b200.h)
+// Deterministic cross-block reductions.  A kernel that sums per-block partials into a gradient writes them to a scratch
+// area and the LAST block to finish adds them up in block order (atomicAdd would sum in arrival order, so two runs of the
+// same step would differ in the last bits and a training run would drift).  Kernels on one stream run one after the
+// other, so each stream the handle sees gets its own scratch area (allocated with the handle; a CUDA graph keeps the
+// capture streams' areas).
+// ---------------------------------------------------------------------------
+constexpr int PD_SCRATCH_SLOTS = 8;             // distinct streams per handle
+constexpr long PD_SCRATCH_FLOATS = 4L << 20;    // partials per stream (16 MB)
+constexpr int PD_SCRATCH_TICKETS = 4096;        // reduction groups per launch
+struct PdScratch {
+    cudaStream_t stream;
+    int used;
+    float* ws;
+    unsigned* tickets;          // all zero between launches: the last block of a group resets its ticket
+};
+
+// ---------------------------------------------------------------------------
+// Handle: host-side state plus the reduction scratch areas
 // ---------------------------------------------------------------------------
 struct pd_handle {
     int device;
     int num_sms;
-    int gemm_impl;            // PD_GEMM_TCGEN05 / PD_GEMM_SIMT
+    int gemm_impl;            // PD_GEMM_TC / PD_GEMM_SIMT
     int max_smem_optin;
     long launches;            // kernels launched through this handle
     char err[512];
     void* encode_tiled;       // cuTensorMapEncodeTiled entry point
     void* encode_im2col;      // cuTensorMapEncodeIm2col entry point (lazy)
     int gemm_smem_configured;
-    int gemm_2cta;            // allow the cta_group::2 256x256 kernel for large problems
-    int gemm_2cta_min_m;      // smallest M that goes to the 2-CTA kernel (PD_GEMM_2CTA_MINM, default 384: three of four 128-row tiles real)
     int fuse_actbwd;          // ELU backward + bias gradient inside the producing GEMM / col2im (PD_B200_FUSE_ACTBWD=0: separate pass)
-    int gemm_2cta_k2;         // 2-CTA kernel, K-major operands: two k-chunks per 3-D TMA box (opt-in: PD_GEMM_2CTA_K2=1)
-    int gemm_plain_m2;        // tall plain GEMMs with N <= 128 on the M2 instantiation (opt-in PD_GEMM_PLAIN_M2=1 / 2: faster alone, step 23.99 vs 23.90 ms)
-    int gemm_conv_m2;         // pd_conv_gemm mode 1: two 128-pixel tiles per weight box (PD_GEMM_CONV_M2=0 disables)
-    int gemm_conv_2cta;       // pd_conv_gemm mode 1 on the 2-CTA kernel (PD_GEMM_CONV_2CTA=0: 1-CTA 128x128 tiles)
-    int gemm_conv_k64;        // pd_conv_gemm modes 2 / 3 with 64-pixel k-blocks (PD_GEMM_CONV_K64=0: 32)
-    int gemm_mn3;             // MN-major operands as one 3-D TMA box per tile (PD_GEMM_MN3=0: four 2-D boxes, the round-1 form)
-    int gemm2_smem_configured;
     int round_ops;            // round tensor-core operands to tf32 (rna) where they are produced
     int k1_configured;        // persistent RSSM kernels: shared-memory opt-in done on THIS handle's device
     int k1_ctas;              // ... and the co-resident grid they launch (one CTA per SM)
     int k1b_configured;
     int k1b_ctas;
+    PdScratch scratch[PD_SCRATCH_SLOTS];
 };
+
+// The scratch area of `stream` (PD_OK), or an error when the handle has seen more streams than it has areas or the
+// launch needs more than one area holds.
+int pd_scratch(pd_handle* h, cudaStream_t stream, long nfloats, int ngroups, float** ws, unsigned** tickets);
 
 // Launch wrappers run on the handle's device whatever the caller's current device is (and put it back).
 struct PdDeviceGuard {
@@ -118,6 +131,21 @@ __device__ __forceinline__ float pd_softplus(float x) {
     return x > 20.f ? x : log1pf(expf(x));
 }
 
+// Called by every thread of every block of a reduction group of n blocks after the block wrote its partials: true in the
+// last block to arrive, which then sees all partials (read them with __ldcg) and resets the group's ticket.
+__device__ __forceinline__ bool pd_last_block(unsigned* ticket, unsigned n) {
+    __shared__ unsigned s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0 && threadIdx.y == 0) {
+        s_last = atomicAdd(ticket, 1u) == n - 1;
+        if (s_last) atomicExch(ticket, 0u);
+    }
+    __syncthreads();
+    if (s_last) __threadfence();
+    return s_last;
+}
+
 __device__ __forceinline__ float pd_warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -146,7 +174,7 @@ __device__ __forceinline__ float pd_block_sum(float v, float* sh /* >= 33 floats
 }
 
 // ---------------------------------------------------------------------------
-// GEMM epilogue shared by the tcgen05 and the SIMT kernels
+// GEMM epilogue shared by the tensor-core and the SIMT kernels
 // ---------------------------------------------------------------------------
 struct PdEpilogue {
     float* C;
@@ -157,15 +185,12 @@ struct PdEpilogue {
     int r_div;
     int act;             // PD_ACT_NONE / PD_ACT_ELU
     int round_out;       // round result to tf32 precision
-    int accumulate;      // 0: C = v ; 1: atomicAdd(C, v) (split-K safe, no bias/act)
-    int c_zeroed;        // caller cleared C already (lets a skinny-M split-K launch skip its memset)
+    int accumulate;      // 0: C = v ; 1: C += v (one addition per element and launch, no bias/act)
     int c_f16;           // C is an fp16 matrix (ldc in halfs): the epilogue converts and stores rows with vector stores
     // backward through the ELU that FOLLOWED the layer whose input gradient this GEMM produces (pd_gemm_actbwd):
-    // v *= elu'(dact[m, n]) (dact = that layer's saved output), then dbias[n] += sum_m v — what pd_bias_act_bwd does in a
-    // separate pass over C
+    // v *= elu'(dact[m, n]) (dact = that layer's saved output); the bias gradient is a column sum of C afterwards
     const float* dact;
     long lddact;
-    float* dbias;
 };
 
 __device__ __forceinline__ float pd_epi_value(const PdEpilogue& e, int row, int col, float acc) {

@@ -157,7 +157,8 @@ __global__ void col2im_v4_kernel(long total4, int Hin, int Win, int Hout, int Wo
 __global__ void __launch_bounds__(192) col2im_actbwd_kernel(long total4, int Hin, int Win, int Hout, int Wout, int C4, int k,
                                                            const float* __restrict__ col, long ldcol,
                                                            const float* __restrict__ dact, int round_out,
-                                                           float* __restrict__ out, float* dbias) {
+                                                           float* __restrict__ out, float* dbias, float* ws,
+                                                           unsigned* tickets) {
     const int Cc = C4 * 4;
     const int c4 = threadIdx.x % C4;
     float4 bs = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -193,14 +194,21 @@ __global__ void __launch_bounds__(192) col2im_actbwd_kernel(long total4, int Hin
         if (round_out) { acc.x = pd_tf32(acc.x); acc.y = pd_tf32(acc.y); acc.z = pd_tf32(acc.z); acc.w = pd_tf32(acc.w); }
         *reinterpret_cast<float4*>(out + pix * Cc + c4 * 4) = acc;
     }
+    if (!dbias) return;
     __shared__ float4 sh[192];
     sh[threadIdx.x] = bs;
     __syncthreads();
-    if (threadIdx.x < C4 && dbias) {
+    if (threadIdx.x < C4) {                    // block partials -> ws[block][Cc]; the last block adds them in block order
         float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int m = threadIdx.x; m < 192; m += C4) { s4.x += sh[m].x; s4.y += sh[m].y; s4.z += sh[m].z; s4.w += sh[m].w; }
-        atomicAdd(dbias + c4 * 4, s4.x); atomicAdd(dbias + c4 * 4 + 1, s4.y);
-        atomicAdd(dbias + c4 * 4 + 2, s4.z); atomicAdd(dbias + c4 * 4 + 3, s4.w);
+        *reinterpret_cast<float4*>(ws + (long)blockIdx.x * Cc + c4 * 4) = s4;
+    }
+    if (pd_last_block(tickets, gridDim.x)) {
+        for (int c = threadIdx.x; c < Cc; c += blockDim.x) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(ws + (long)b * Cc + c);
+            dbias[c] += s;
+        }
     }
 }
 
@@ -298,9 +306,10 @@ col2im_imgloss_kernel(int Hin, int Win, int Hout, int Wout, int Cc, int k, const
     if (threadIdx.x == 0) loss[n] = 0.5f * s;
 }
 
-// dy <- dy * act'(y);  db[c] += sum_rows.  blockDim = (32, 8): a warp owns 32 consecutive columns.
+// dy <- dy * act'(y);  db[c] += sum_rows.  blockDim = (32, 8): a warp owns 32 consecutive columns; the blocks of one
+// column group (blockIdx.x) write their partials to ws and the last of them adds them to db in blockIdx.y order.
 __global__ void bias_act_bwd_kernel(long M, int N, float* __restrict__ dy, long lddy, const float* __restrict__ y,
-                                    long ldy, int act, float* db, int round_out) {
+                                    long ldy, int act, float* db, int round_out, float* ws, unsigned* tickets) {
     const int c = blockIdx.x * 32 + threadIdx.x;
     float acc = 0.f;
     if (c < N) {
@@ -313,14 +322,21 @@ __global__ void bias_act_bwd_kernel(long M, int N, float* __restrict__ dy, long 
             acc += g;
         }
     }
+    if (!db) return;
     __shared__ float sh[8][33];
     sh[threadIdx.y][threadIdx.x] = acc;
     __syncthreads();
-    if (threadIdx.y == 0 && c < N && db) {
+    float* part = ws + (long)blockIdx.x * gridDim.y * 32 + threadIdx.x;
+    if (threadIdx.y == 0) {
         float s = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) s += sh[i][threadIdx.x];
-        atomicAdd(db + c, s);
+        part[blockIdx.y * 32] = s;
+    }
+    if (pd_last_block(tickets + blockIdx.x, gridDim.y) && threadIdx.y == 0 && c < N) {
+        float s = 0.f;
+        for (unsigned b = 0; b < gridDim.y; ++b) s += __ldcg(part + b * 32);
+        db[c] += s;
     }
 }
 
@@ -432,8 +448,16 @@ int pd_col2im_actbwd(pd_handle* h, int NB, int Hin, int Win, int Hout, int Wout,
         if (rc) return rc;
         return pd_bias_act_bwd(h, (long)NB * Hout * Wout, Cc, out, Cc, dact, Cc, PD_ACT_ELU, dbias, stream);
     }
-    col2im_actbwd_kernel<<<grid_for(total / 4, 192, h->num_sms), 192, 0, (cudaStream_t)stream>>>(
-        total / 4, Hin, Win, Hout, Wout, Cc / 4, k, col, ldcol, dact, h->round_ops, out, dbias);
+    int grid = grid_for(total / 4, 192, h->num_sms);
+    float* ws = nullptr;
+    unsigned* tk = nullptr;
+    if (dbias) {
+        if ((long)grid * Cc > PD_SCRATCH_FLOATS) grid = (int)(PD_SCRATCH_FLOATS / Cc);   // grid-stride loop: any grid works
+        int rc = pd_scratch(h, (cudaStream_t)stream, (long)grid * Cc, 1, &ws, &tk);
+        if (rc) return rc;
+    }
+    col2im_actbwd_kernel<<<grid, 192, 0, (cudaStream_t)stream>>>(
+        total / 4, Hin, Win, Hout, Wout, Cc / 4, k, col, ldcol, dact, h->round_ops, out, dbias, ws, tk);
     PD_CHECK_LAUNCH(h, "col2im_actbwd");
     return PD_OK;
 }
@@ -470,7 +494,13 @@ int pd_bias_act_bwd(pd_handle* h, long M, int N, float* dy, long lddy, const flo
     if (cap < 1) cap = 1;
     if (gy > cap) gy = cap;
     dim3 grid((N + 31) / 32, (unsigned)gy);
-    bias_act_bwd_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(M, N, dy, lddy, y, ldy, act, db, h->round_ops);
+    float* ws = nullptr;
+    unsigned* tk = nullptr;
+    if (db) {
+        int rc = pd_scratch(h, (cudaStream_t)stream, (long)grid.x * grid.y * 32, (int)grid.x, &ws, &tk);
+        if (rc) return rc;
+    }
+    bias_act_bwd_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(M, N, dy, lddy, y, ldy, act, db, h->round_ops, ws, tk);
     PD_CHECK_LAUNCH(h, "bias_act_bwd");
     return PD_OK;
 }

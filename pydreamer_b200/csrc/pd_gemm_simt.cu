@@ -1,7 +1,7 @@
-// pd_gemm_simt.cu — plain fp32 CUDA-core tile GEMM with the same contract as the tcgen05 kernel.
+// pd_gemm_simt.cu — plain fp32 CUDA-core tile GEMM with the same contract as the tensor-core kernel.
 // It exists as the validation arm for tests (PD_GEMM_SIMT): every composite test can be run with
 // either implementation, which separates "is the tensor-core pipeline right" from "is the model
-// math right".  Not used by the product path (pd_create selects PD_GEMM_TCGEN05).
+// math right".  Not used by the product path (pd_create selects PD_GEMM_TC).
 #include "pd_common.cuh"
 #include <cuda_fp16.h>
 
@@ -89,9 +89,9 @@ gemv_rows_kernel(int M, int N, int K, const float* __restrict__ A, long lda, con
 }
 
 // C[m, n] += sum_k A[k, m] * B[k, n]  for M <= 4 (weight gradient of a scalar head): blockDim (32, 8), a warp owns
-// 32 consecutive n; rows k are strided over blockIdx.y.
+// 32 consecutive n; rows k are strided over blockIdx.y, whose partials the last block of the column group adds in order.
 __global__ void wcolsum_kernel(int M, int N, long K, const float* __restrict__ A, long lda, const float* __restrict__ B,
-                               long ldb, float* C, long ldc) {
+                               long ldb, float* C, long ldc, float* ws, unsigned* tickets) {
     const int n = blockIdx.x * 32 + threadIdx.x;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     if (n < N) {
@@ -105,12 +105,20 @@ __global__ void wcolsum_kernel(int M, int N, long K, const float* __restrict__ A
 #pragma unroll
     for (int m = 0; m < 4; ++m) sh[m][threadIdx.y][threadIdx.x] = acc[m];
     __syncthreads();
-    if (threadIdx.y == 0 && n < N) {
+    float* part = ws + (long)blockIdx.x * gridDim.y * 128 + threadIdx.x;      // [y][m][32]
+    if (threadIdx.y == 0) {
         for (int m = 0; m < M; ++m) {
             float s = 0.f;
 #pragma unroll
             for (int i = 0; i < 8; ++i) s += sh[m][i][threadIdx.x];
-            atomicAdd(C + (long)m * ldc + n, s);
+            part[blockIdx.y * 128 + m * 32] = s;
+        }
+    }
+    if (pd_last_block(tickets + blockIdx.x, gridDim.y) && threadIdx.y == 0 && n < N) {
+        for (int m = 0; m < M; ++m) {
+            float s = 0.f;
+            for (unsigned b = 0; b < gridDim.y; ++b) s += __ldcg(part + b * 128 + m * 32);
+            C[(long)m * ldc + n] += s;
         }
     }
 }
@@ -129,24 +137,23 @@ int pd_gemm_simt_launch(pd_handle* h, int M, int N, int K, const float* A, long 
             long cap = (long)h->num_sms * 8 / ((N + 31) / 32);
             if (cap < 1) cap = 1;
             if (gy > cap) gy = cap;
-            wcolsum_kernel<<<dim3((N + 31) / 32, (unsigned)gy), dim3(32, 8), 0, stream>>>(M, N, K, A, lda, B, ldb, epi.C, epi.ldc);
+            float* ws;
+            unsigned* tk;
+            const int gx = (N + 31) / 32;
+            int rc = pd_scratch(h, stream, (long)gx * gy * 128, gx, &ws, &tk);
+            if (rc) return rc;
+            wcolsum_kernel<<<dim3(gx, (unsigned)gy), dim3(32, 8), 0, stream>>>(M, N, K, A, lda, B, ldb, epi.C, epi.ldc, ws, tk);
             PD_CHECK_LAUNCH(h, "wcolsum_kernel");
             return PD_OK;
         }
     }
     long sAm = a_mn ? 1 : lda, sAk = a_mn ? lda : 1;
     long sBn = b_mn ? 1 : ldb, sBk = b_mn ? ldb : 1;
-    int gx = pd_cdiv(N, TN), gy = pd_cdiv(M, TM), gz = 1;
-    if (epi.accumulate) {
-        int tiles = gx * gy;
-        gz = (2 * h->num_sms) / tiles;
-        int maxz = pd_cdiv(K, 256);
-        if (gz > maxz) gz = maxz;
-        if (gz < 1) gz = 1;
-    }
-    int kchunk = pd_cdiv(pd_cdiv(K, gz), TK) * TK;
-    gz = pd_cdiv(K, kchunk);
-    dim3 grid(gx, gy, gz);
+    // one block per output tile over the whole of K: an accumulating launch adds each element once (no split-K, whose
+    // atomic partial sums would land in arrival order)
+    int gx = pd_cdiv(N, TN), gy = pd_cdiv(M, TM);
+    int kchunk = pd_cdiv(K, TK) * TK;
+    dim3 grid(gx, gy, 1);
     pd_gemm_simt_kernel<<<grid, 256, 0, stream>>>(M, N, K, A, sAm, sAk, B, sBn, sBk, epi, kchunk);
     PD_CHECK_LAUNCH(h, "pd_gemm_simt_kernel");
     return PD_OK;

@@ -114,7 +114,7 @@ __device__ __forceinline__ void producer_wait_barrier(const unsigned* ctr, unsig
 }
 
 // Diagnostic: CTA 0 accumulates the nanoseconds between consecutive laps per phase slot into ws_barrier[2 + 2 * slot]
-// (7 uint64 counters, read by tools/k1_time.py / k1b_time.py); one clock read per phase, no effect on the result.
+// (7 uint64 counters); one clock read per phase, no effect on the result.
 struct PhaseClock {
     unsigned long long last;
     unsigned long long* acc;
@@ -167,7 +167,7 @@ struct Job {
     int kcol0, nkb, x2_from;
     // Grouped weight boxes (ngop > 0): the SAME ntile tiles fetched by a few larger TMA operations instead of one 2 KB box per
     // tile — op o fills tiles gdst[o].. from rows grow[o].. of gmap[o]; g3d[o]: a 3-D map (k, row within gate, gate) whose box
-    // spans all gates (tools/microbench/tma_box_rate.cu: small boxes cost almost as much as large ones).
+    // spans all gates (a TMA operation costs about the same for a small box as for a large one).
     int ngop;
     const CUtensorMap* gmap[3];
     int grow[3], gdst[3], g3d[3];
@@ -325,92 +325,6 @@ __device__ void consume_f16(Ring<MAXT, XB>& ring, const Job<MAXT>& j, int tile0,
         if (lane == 0) mbar_arrive(ring.empty + n % NSTAGE);
     }
     ring.n += j.nkb;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// tcgen05 (5th-generation tensor core) contraction over the same ring: the stage's weight tiles form UMMA A tiles of 128
-// rows (eight 16-row TMA boxes each = sixteen 8-row x 128-byte SWIZZLE_128B atoms, exactly the canonical K-major layout the
-// tcgen05 GEMM of pd_gemm_tcgen05.cu uses), the 64-row fp16 activation box is the K-major B tile (N = 64), accumulators live
-// in TMEM (lane = weight row, column = batch row).  One elected thread issues the MMAs; the stage is released by
-// tcgen05.commit (one arrival when its MMAs have retired) plus one plain arrival from each of the other consumer warps.
-// ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_c, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_c), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tc_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// UMMA shared-memory matrix descriptor, K-major SWIZZLE_128B tile (cute SmemDescriptor bit layout, as in pd_gemm_tcgen05.cu):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (1024 B between 8-row groups) |
-//   [46,48) version=1 | [61,64) layout 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((16u >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// instruction descriptor: D = F32, A = B = F16, both K-major, N, M = 128
-__device__ __forceinline__ uint32_t umma_idesc_f16(int N) { return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24); }
-
-// All consumer warps walk the job's stages; the elected thread issues, per stage, 4 k16 steps x NUT UMMA tiles
-// (accumulators at TMEM columns tmem + ut * NCOL) and commits the stage; after the last stage it commits `accbar`, which every
-// consumer thread then waits for (parity `accpar`) before reading TMEM.
-template <int NUT, int NCOL, int MAXT, int XB>
-__device__ void consume_umma(Ring<MAXT, XB>& ring, const Job<MAXT>& j, uint32_t tmem, uint64_t* accbar, uint32_t accpar,
-                             bool finish = true) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t idesc = umma_idesc_f16(NCOL);
-    for (int kb = 0; kb < j.nkb; ++kb) {
-        const uint32_t n = ring.n + kb;
-        mbar_wait(ring.full + n % NSTAGE, (n / NSTAGE) & 1);
-        if (warp == 0) {
-            if (lane == 0) {
-                tc_fence_after();
-                const uint32_t sa = s_u32(ring.stage(n)), sb = s_u32(ring.xbase(n));
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    const uint64_t bd = umma_desc(sb + ks * 32);
-#pragma unroll
-                    for (int ut = 0; ut < NUT; ++ut)
-                        tc_mma_f16(tmem + (uint32_t)(ut * NCOL), umma_desc(sa + ut * 8 * A_TILE + ks * 32), bd, idesc,
-                                   (kb > 0 || ks > 0) ? 1u : 0u);
-                }
-                tc_commit(ring.empty + n % NSTAGE);                 // one arrival when these MMAs have retired
-                if (finish && kb == j.nkb - 1) tc_commit(accbar);   // (finish = false: more MMAs of this phase follow, into
-                                                                    //  other TMEM columns; the last job's commit covers them all)
-            }
-            __syncwarp();
-        } else {
-            if (lane == 0) mbar_arrive(ring.empty + n % NSTAGE);    // this warp does not read the stage
-        }
-    }
-    ring.n += j.nkb;
-    if (finish && j.nkb > 0) {
-        mbar_wait(accbar, accpar);
-        tc_fence_after();
-    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

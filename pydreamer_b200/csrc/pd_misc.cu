@@ -73,8 +73,9 @@ __global__ void reset_mask_kernel(int T, int B, int I, const uint8_t* __restrict
         mask[i] = reset[tb] ? 0.f : 1.f;
     }
 }
-// out[c] += sum_rows x[r, c] ; blockDim (32, 8)
-__global__ void colsum_kernel(long M, int N, const float* __restrict__ x, long ldx, float* out) {
+// out[c] += sum_rows x[r, c] ; blockDim (32, 8); partials of the blocks of one column group are added in blockIdx.y order
+// by the last of them (pd_last_block)
+__global__ void colsum_kernel(long M, int N, const float* __restrict__ x, long ldx, float* out, float* ws, unsigned* tickets) {
     const int c = blockIdx.x * 32 + threadIdx.x;
     float acc = 0.f;
     if (c < N)
@@ -83,11 +84,17 @@ __global__ void colsum_kernel(long M, int N, const float* __restrict__ x, long l
     __shared__ float sh[8][33];
     sh[threadIdx.y][threadIdx.x] = acc;
     __syncthreads();
-    if (threadIdx.y == 0 && c < N) {
+    float* part = ws + (long)blockIdx.x * gridDim.y * 32 + threadIdx.x;
+    if (threadIdx.y == 0) {
         float s = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) s += sh[i][threadIdx.x];
-        atomicAdd(out + c, s);
+        part[blockIdx.y * 32] = s;
+    }
+    if (pd_last_block(tickets + blockIdx.x, gridDim.y) && threadIdx.y == 0 && c < N) {
+        float s = 0.f;
+        for (unsigned b = 0; b < gridDim.y; ++b) s += __ldcg(part + b * 32);
+        out[c] += s;
     }
 }
 
@@ -434,7 +441,11 @@ int pd_colsum(pd_handle* h, long M, int N, const float* x, long ldx, float* out,
     if (cap < 1) cap = 1;
     if (gy > cap) gy = cap;
     dim3 grid((N + 31) / 32, (unsigned)gy);
-    colsum_kernel<<<grid, block, 0, S(stream)>>>(M, N, x, ldx, out);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), (long)grid.x * grid.y * 32, (int)grid.x, &ws, &tk);
+    if (rc) return rc;
+    colsum_kernel<<<grid, block, 0, S(stream)>>>(M, N, x, ldx, out, ws, tk);
     PD_CHECK_LAUNCH(h, "colsum");
     return PD_OK;
 }

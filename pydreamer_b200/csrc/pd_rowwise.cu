@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(128)
 ln_elu_bwd_kernel(int M, int N, const float* __restrict__ dy, long lddy, const float* __restrict__ x, long ldx,
                   const float* __restrict__ y, long ldy, const float* __restrict__ gamma,
                   const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dx,
-                  long lddx, float* dgamma, float* dbeta, float* dbias, int round_out) {
+                  long lddx, float* dgamma, float* dbeta, float* dbias, int round_out, float* ws, unsigned* tickets) {
     __shared__ float sh[3][32 * MAXV];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int c = threadIdx.x; c < 32 * MAXV; c += 128) { sh[0][c] = 0.f; sh[1][c] = 0.f; sh[2][c] = 0.f; }
@@ -101,17 +101,33 @@ ln_elu_bwd_kernel(int M, int N, const float* __restrict__ dy, long lddy, const f
             }
         }
     }
+    // parameter gradients in a fixed order: the four warps in turn into shared memory, the block's partials to
+    // ws[block][3][N], the last block adds them up in block order
+    for (int w = 0; w < 4; ++w) {
+        if (warp == w) {
 #pragma unroll
-    for (int i = 0; i < MAXV; ++i) {
-        atomicAdd(&sh[0][lane + 32 * i], pg[i]);
-        atomicAdd(&sh[1][lane + 32 * i], pb[i]);
-        atomicAdd(&sh[2][lane + 32 * i], px[i]);
+            for (int i = 0; i < MAXV; ++i) {
+                sh[0][lane + 32 * i] += pg[i];
+                sh[1][lane + 32 * i] += pb[i];
+                sh[2][lane + 32 * i] += px[i];
+            }
+        }
+        __syncthreads();
     }
-    __syncthreads();
+    float* part = ws + (long)blockIdx.x * 3 * N;
     for (int c = threadIdx.x; c < N; c += 128) {
-        atomicAdd(dgamma + c, sh[0][c]);
-        atomicAdd(dbeta + c, sh[1][c]);
-        if (dbias) atomicAdd(dbias + c, sh[2][c]);
+        part[c] = sh[0][c]; part[N + c] = sh[1][c]; part[2 * N + c] = sh[2][c];
+    }
+    if (pd_last_block(tickets, gridDim.x)) {
+        for (int c = threadIdx.x; c < N; c += 128) {
+            float g = 0.f, b = 0.f, d = 0.f;
+            for (unsigned k = 0; k < gridDim.x; ++k) {
+                const float* p = ws + (long)k * 3 * N;
+                g += __ldcg(p + c); b += __ldcg(p + N + c); d += __ldcg(p + 2 * N + c);
+            }
+            dgamma[c] += g; dbeta[c] += b;
+            if (dbias) dbias[c] += d;
+        }
     }
 }
 
@@ -151,7 +167,8 @@ __global__ void __launch_bounds__(256)
 ln_elu_bwd_row_kernel(int N, const float* __restrict__ dy, long lddy, const float* __restrict__ x, long ldx,
                       const float* __restrict__ y, long ldy, const float* __restrict__ gamma,
                       const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dx,
-                      long lddx, float* dgamma, float* dbeta, float* dbias, int round_out) {
+                      long lddx, float* dgamma, float* dbeta, float* dbias, int round_out, float* ws,
+                      unsigned* tickets) {
     __shared__ float sh[33];
     const int row = blockIdx.x, t = threadIdx.x;
     const float mean = mean_in[row], rstd = rstd_in[row];
@@ -174,9 +191,19 @@ ln_elu_bwd_row_kernel(int N, const float* __restrict__ dy, long lddy, const floa
         if (c < N) {
             float d = rstd * (dxh[i] - c1 - xh[i] * c2);
             dx[(long)row * lddx + c] = pd_round_if(d, round_out);
-            atomicAdd(dgamma + c, g[i] * xh[i]);
-            atomicAdd(dbeta + c, g[i]);
-            if (dbias) atomicAdd(dbias + c, d);
+            float* part = ws + (long)row * 3 * N;            // this row's parameter-gradient terms
+            part[c] = g[i] * xh[i]; part[N + c] = g[i]; part[2 * N + c] = d;
+        }
+    }
+    if (pd_last_block(tickets, gridDim.x)) {                 // the last row block adds all rows' terms in row order
+        for (int c = t; c < N; c += 256) {
+            float sg = 0.f, sb = 0.f, sd = 0.f;
+            for (unsigned r = 0; r < gridDim.x; ++r) {
+                const float* p = ws + (long)r * 3 * N;
+                sg += __ldcg(p + c); sb += __ldcg(p + N + c); sd += __ldcg(p + 2 * N + c);
+            }
+            dgamma[c] += sg; dbeta[c] += sb;
+            if (dbias) dbias[c] += sd;
         }
     }
 }
@@ -379,17 +406,23 @@ int pd_ln_elu_bwd(pd_handle* h, int M, int N, const float* dy, long lddy, const 
                   float* dgamma, float* dbeta, float* dbias, void* stream) {
     PD_REQUIRE(h, N >= 1 && N <= 1024, "pd_ln_elu_bwd: N=%d unsupported (1..1024)", N);
     cudaStream_t s = (cudaStream_t)stream;
+    float* ws;
+    unsigned* tk;
     if (M <= 256) {
+        int rc = pd_scratch(h, s, (long)M * 3 * N, 1, &ws, &tk);
+        if (rc) return rc;
         ln_elu_bwd_row_kernel<<<M, 256, 0, s>>>(N, dy, lddy, x, ldx, y, ldy, gamma, mean, rstd, dx, lddx, dgamma, dbeta,
-                                               dbias, h->round_ops);
+                                               dbias, h->round_ops, ws, tk);
         PD_CHECK_LAUNCH(h, "ln_elu_bwd_row");
         return PD_OK;
     }
     int grid = pd_cdiv(M, 4);
     int cap = 2 * h->num_sms;
     if (grid > cap) grid = cap;
-    if (N <= 416) ln_elu_bwd_kernel<13><<<grid, 128, 0, s>>>(M, N, dy, lddy, x, ldx, y, ldy, gamma, mean, rstd, dx, lddx, dgamma, dbeta, dbias, h->round_ops);
-    else          ln_elu_bwd_kernel<32><<<grid, 128, 0, s>>>(M, N, dy, lddy, x, ldx, y, ldy, gamma, mean, rstd, dx, lddx, dgamma, dbeta, dbias, h->round_ops);
+    int rc = pd_scratch(h, s, (long)grid * 3 * N, 1, &ws, &tk);
+    if (rc) return rc;
+    if (N <= 416) ln_elu_bwd_kernel<13><<<grid, 128, 0, s>>>(M, N, dy, lddy, x, ldx, y, ldy, gamma, mean, rstd, dx, lddx, dgamma, dbeta, dbias, h->round_ops, ws, tk);
+    else          ln_elu_bwd_kernel<32><<<grid, 128, 0, s>>>(M, N, dy, lddy, x, ldx, y, ldy, gamma, mean, rstd, dx, lddx, dgamma, dbeta, dbias, h->round_ops, ws, tk);
     PD_CHECK_LAUNCH(h, "ln_elu_bwd");
     return PD_OK;
 }

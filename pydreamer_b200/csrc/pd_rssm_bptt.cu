@@ -8,7 +8,7 @@
 // -> gemm  of pydreamer_b200/dreamer.py (_wm_backward) and writes exactly the tensors that chain writes (dpost, dy2, dgi, dgh,
 // dx1: the operands of the batched weight-gradient GEMMs that follow) plus the LayerNorm / bias gradients it accumulates.
 //
-// Structure (B200: 148 SMs, one CTA per SM, cooperative launch):
+// Structure (one CTA per SM, 132 on an H100, cooperative launch):
 //   * 8 consumer warps + 1 producer warp.  The producer streams operands with TMA (cp.async.bulk.tensor.2d, 128-byte
 //     swizzle) into a 4-stage shared-memory ring guarded by full / empty mbarriers; a stage = one 64-wide k-block of up to
 //     six 16-row weight tiles (fp16) and up to four 64-row x 32-float boxes of the gradient operand (fp32).
@@ -17,7 +17,7 @@
 //   * contractions: out[rows, batch] = W^T[rows, K] . X[batch, K]^T on the legacy tensor path
 //     (mma.sync.m16n8k8 tf32): weight fragments come from fp16 tiles (ldmatrix, exact fp16 -> tf32 unpack), the gradient
 //     operand stays fp32 / tf32-rounded — gradients need fp32's exponent range, so fp16 operands are not an option here,
-//     and both operands carry 10 mantissa bits exactly like the TF32 tcgen05 GEMMs of the launch chain.
+//     and both operands carry 10 mantissa bits exactly like the TF32 tensor-core GEMMs of the launch chain.
 //   * per timestep six dependent phases, separated by grid barriers (one atomic + one polled word in L2):
 //       P9+P1  latent-group owners : dz_{t} = dx1_{t+1} W_z (kept in smem) -> straight-through softmax backward + KL term -> dpost_t
 //       P2     (row-group, k-slice): dpin = dpost_t W_pm          partial sums over 4 k-slices -> global

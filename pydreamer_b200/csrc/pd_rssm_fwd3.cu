@@ -16,23 +16,19 @@
 //   C'  batch-row owners      : y2 = sum of partials + b_ph + ea_t ; LayerNorm + ELU -> pin
 //   D   latent-group owners   : logits of group g for a quarter of the batch rows = pin . W_pm^T ; softmax ; argmax(p / q)
 // Weights are fp16, activations fp16 (za, h', pin: the same 10 mantissa bits as the TF32 chain), accumulation fp32.
-// The two wide contractions (B, C) run on the 5th-generation tensor cores: tcgen05.mma.kind::f16, M = 128 weight rows (eight
-// 16-row TMA boxes form one UMMA A tile), N = 64 batch rows, accumulators in TMEM, read back with tcgen05.ld for the
-// epilogues (r02 phase clocks of the mma.sync version: phase C spent 8.6 of its 11.4 us issuing legacy HMMA).  The small
-// logits contraction of phase D (32 rows x 16 batch rows) stays on mma.sync.
+// All contractions run on mma.sync m16n8k16 with ldmatrix fragments (consume_f16, pd_k1_pipe.cuh): the weight rows are the
+// MMA's M side (16-row tiles), the batch rows its N side, accumulators in registers.
 //
 // Batch rows beyond one 64-row MMA operand (IWAE: BI = B x iwae_samples, world.py:60-68 repeats every sequence I times) run in
-// the MULTI instantiation: phases B and C repeat their contraction per block of 64 rows into separate TMEM columns (all
-// blocks' MMAs are issued back to back, one commit, then the epilogues block by block), phase D takes 64 rows per pass with
-// all eight warps, and the row owners of A / C' stride over the rows by the grid size.  The single-block instantiation is
-// the round-2 kernel unchanged (same-box A/B: a run-time block loop around its phases cost 0.38 ms on the Atari shape).
+// the MULTI instantiation: phases B and C repeat their contraction and epilogue per block of 64 rows, phase D takes 64 rows
+// per pass with all eight warps, and the row owners of A / C' stride over the rows by the grid size.
 #include "pd_k1_pipe.cuh"
 
 namespace {
 using namespace k1;
 
 constexpr int MAXT = 16;                       // phase C: 3 gates x 4 tiles of W_hh rows + 2 tiles of W_ph rows = 14 of the
-                                               // 16 box slots of two 128-row UMMA tiles
+                                               // 16 box slots
 typedef Ring<MAXT, 1> RingF;
 typedef Job<MAXT> JobF;
 constexpr int OFF_BAR = RingF::BYTES;
@@ -42,10 +38,8 @@ constexpr int HB = 256;                                     // batch rows the MU
 constexpr int OFF_HC = OFF_SIDX + 256;                      // [16][BROWS or HB] floats: masked h of my units (input of the next step)
 constexpr int OFF_PART = OFF_HC + 16 * HB * 4;              // [2][1024] floats: phase A gather halves
 constexpr int OFF_LOG = OFF_PART + 2 * 1024 * 4;            // [16 or 64][32] floats: phase D logits of my rows
-constexpr int OFF_GI = OFF_LOG + 64 * 32 * 4;               // [48][65] floats: phase B gi of my units (from TMEM, for the gate math)
-constexpr int OFF_TM = OFF_GI + 48 * 65 * 4;                // accumulator-ready mbarrier (8 B) + TMEM base address (4 B)
-constexpr int SMEM_BYTES = OFF_TM + 64;
-// TMEM columns: two UMMA tiles x 64 batch columns per block of batch rows (128, or all 512 with four blocks)
+constexpr int OFF_GI = OFF_LOG + 64 * 32 * 4;               // [48][65] floats: phase B gi of my units (for the gate math)
+constexpr int SMEM_BYTES = OFF_GI + 48 * 65 * 4;
 constexpr int KSPLIT = 4;
 
 struct FwdMaps {
@@ -90,7 +84,6 @@ __device__ void ln_elu_row(float (&v)[4], int N, const float* __restrict__ gamma
 template <bool MULTI>
 __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_fwd_args a, const __grid_constant__ FwdMaps maps,
                                                                  const int KS, const int GW) {
-    constexpr int TMEM_COLS = MULTI ? 512 : 128;
     constexpr int HS = MULTI ? HB : BROWS;                  // row stride of hcs
     constexpr int DR = MULTI ? 64 : 16;                     // batch rows of one phase-D pass
     extern __shared__ uint8_t smem_raw[];
@@ -101,8 +94,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     float* part = (float*)(smem + OFF_PART);                // [2][Hd]
     float* lgs = (float*)(smem + OFF_LOG);                  // lgs[rb * 32 + class]
     float* gis = (float*)(smem + OFF_GI);                   // gis[(gate * 16 + r) * 65 + b]
-    uint64_t* accbar = (uint64_t*)(smem + OFF_TM);
-    uint32_t* tmem_slot = (uint32_t*)(smem + OFF_TM + 8);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool producer = warp == NCW;
@@ -116,12 +107,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
 
     RingF ring;
     ring.init(smem, (uint64_t*)(smem + OFF_BAR));
-    if (tid == 0) mbar_init(accbar, 1);
-    if (warp == 0) {                                        // TMEM: 128 columns for the whole kernel
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
 
     // ---- static ownership
     const int u4_0 = (int)((long)c * D / P), u4_1 = (int)((long)(c + 1) * D / P), nu = u4_1 - u4_0;   // B: my hidden units
@@ -140,9 +125,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
 
     for (int o = tid; o < nu * BI; o += NT) hcs[(o % nu) * HS + o / nu] = __ldcg(a.hin + (long)(o / nu) * D + u4_0 + o % nu);
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    uint32_t accpar = 0;
 
     auto job_b = [&]() {
         JobF j; j.ntile = nu > 0 ? 3 : 0; j.nx = 1; j.xmap[0] = &maps.za; j.xmap[1] = &maps.za; j.xrow0 = 0; j.xrows = BROWS; j.xf16 = 1;
@@ -197,36 +179,39 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     auto phase_c = [&](bool want_gh, bool want_y2) {
         const JobF j = job_c();
         if (j.nkb == 0) return;
-        for (int bb = 0; bb < NBB; ++bb) consume_umma<2, 64>(ring, j, tmem + (uint32_t)(bb * 128), accbar, accpar, bb == NBB - 1);
-        accpar ^= 1;
-        // warp w reads UMMA tile (w >> 2), TMEM lane quarter (w & 3): thread = one weight row x 64 batch columns
-        const int ut = warp >> 2, quarter = warp & 3;
-        const int urow = quarter * 32 + lane, slot = ut * 8 + (urow >> 4), rr = urow & 15;
-        float* dst = nullptr;                                   // element b of my row goes to dst[b * bstride]: partial planes
-                                                                // [ks][b][row], lanes = consecutive rows -> coalesced stores
-        long bstride = 0;
-        if (slot < 12) {
-            const int gate = slot >> 2, u = u6_0 + (slot & 3) * 16 + rr;
-            if (want_gh && u < u6_1) { dst = a.ws_ghpart + (long)ks * BI * D3 + (long)gate * D + u; bstride = D3; }
-        } else if (slot < 14) {
-            const int f = f6_0 + (slot - 12) * 16 + rr;
-            if (want_y2 && f < f6_1) { dst = a.ws_y2part + (long)ks * BI * Hd + f; bstride = Hd; }
-        }
+        // warp w < 7 takes weight tiles 2w, 2w + 1 (tile = gate * 4 + i for W_hh, 12 + i for W_ph) x all 64 batch rows
+        const bool act = warp < 7;
         for (int bb = 0; bb < NBB; ++bb) {
+            float acc[2][8][4];
+            consume_f16<2, 8>(ring, j, 2 * warp, 0, act, acc);
+            if (!act) continue;
+            const int g = lane >> 2, tq = lane & 3;
 #pragma unroll
-            for (int cc = 0; cc < 2; ++cc) {
-                uint32_t r[32];
-                tc_ld_32x32b_x32(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(bb * 128 + ut * 64 + cc * 32), r);
-                if (dst) {
+            for (int i = 0; i < 2; ++i) {
+                const int slot = 2 * warp + i;
 #pragma unroll
-                    for (int jb = 0; jb < 32; ++jb) {
-                        const int b = bb * BROWS + cc * 32 + jb;
-                        if (b < BI) dst[(long)b * bstride] = __uint_as_float(r[jb]);
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int rr = g + 8 * hr;
+                    float* dst = nullptr;                       // element b of this row goes to dst[b * bstride]: partial
+                    long bstride = 0;                           // planes [ks][b][row]
+                    if (slot < 12) {
+                        const int gate = slot >> 2, u = u6_0 + (slot & 3) * 16 + rr;
+                        if (want_gh && u < u6_1) { dst = a.ws_ghpart + (long)ks * BI * D3 + (long)gate * D + u; bstride = D3; }
+                    } else {
+                        const int f = f6_0 + (slot - 12) * 16 + rr;
+                        if (want_y2 && f < f6_1) { dst = a.ws_y2part + (long)ks * BI * Hd + f; bstride = Hd; }
                     }
+                    if (!dst) continue;
+#pragma unroll
+                    for (int jn = 0; jn < 8; ++jn)
+#pragma unroll
+                        for (int x = 0; x < 2; ++x) {
+                            const int b = bb * BROWS + jn * 8 + 2 * tq + x;
+                            if (b < BI) dst[(long)b * bstride] = acc[i][jn][2 * hr + x];
+                        }
                 }
             }
         }
-        tc_fence_before();
     };
 
     // ---- prologue: fp16 h_0 for the TMA reads of the first recurrent product
@@ -300,21 +285,22 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
         {
             const JobF j = job_b();
             if (j.nkb > 0) {
-                for (int bb = 0; bb < NBB; ++bb) consume_umma<1, 64>(ring, j, tmem + (uint32_t)(bb * 64), accbar, accpar, bb == NBB - 1);
-                accpar ^= 1;
               for (int bb = 0; bb < NBB; ++bb) {
                 if (MULTI && bb > 0) cons_sync();                          // gis of the previous block has been read
-                // rows 0..47 of the UMMA tile = (gate, unit): quarters 0 and 1; warps w and w + 4 take 32 batch columns each
-                if ((warp & 3) < 2) {
-                    const int quarter = warp & 3, cc = warp >> 2, urow = quarter * 32 + lane;
-                    uint32_t r[32];
-                    tc_ld_32x32b_x32(tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(bb * 64 + cc * 32), r);
-                    if (urow < 48) {
+                // warps 0..3: the three gate tiles x two n8-tiles (16 batch rows) each
+                float acc[3][2][4];
+                const bool act = warp < 4;
+                consume_f16<3, 2>(ring, j, 0, 2 * warp, act, acc);
+                if (act) {
+                    const int g = lane >> 2, tq = lane & 3;
 #pragma unroll
-                        for (int jb = 0; jb < 32; ++jb) gis[urow * 65 + cc * 32 + jb] = __uint_as_float(r[jb]);
-                    }
+                    for (int i = 0; i < 3; ++i)
+#pragma unroll
+                        for (int jn = 0; jn < 2; ++jn)
+#pragma unroll
+                            for (int x = 0; x < 4; ++x)
+                                gis[(i * 16 + g + 8 * (x >> 1)) * 65 + (2 * warp + jn) * 8 + 2 * tq + (x & 1)] = acc[i][jn][x];
                 }
-                tc_fence_before();
                 cons_sync();
                 // gate math: one (unit, batch row) per thread iteration, unit fastest (coalesced global accesses)
                 const int nb = MULTI ? min(BROWS, BI - bb * BROWS) : BI;
@@ -444,9 +430,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
         if (t + 1 < T) grid_barrier(a.ws_barrier, epoch);                       // (5) idx_t complete
         clk.lap(5);
     }
-    tc_fence_before();
-    cons_sync();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
 }
 
 }  // namespace

@@ -1,5 +1,5 @@
 """Drop-in `Dreamer` module: the reference's API (pydreamer/models/dreamer.py:19-230) over hand-written
-sm_100a kernels.
+sm_90a kernels.
 
 What is kept from the reference contract (SURVEY.md §8 b1):
   * ctor `Dreamer(conf)` with the reference's config keys; an nn.Module whose state_dict keys and
@@ -778,8 +778,6 @@ class Dreamer(nn.Module):
     #   1  dream + actor-critic (needs only the detached features) alongside decoder / losses / world-model backward
     #   2  the h·W_hh GEMM of the next step (and its transpose in BPTT) off the per-timestep critical path
     #   4  image-decoder weight gradients alongside the input-gradient chain and BPTT
-    # (Measured, profiles/README.md: 1 is worth 4.5 ms of 36; 2 and 4 are within noise; running the encoder in time
-    #  chunks beside the unroll / BPTT gained nothing - the split-K chain GEMMs already occupy every SM.)
     overlap = int(os.environ.get("PD_B200_OVERLAP", "3"))
     _scratch_ns = ""          # name space of the shared MLP scratch buffers (one per concurrent branch)
 
@@ -790,7 +788,7 @@ class Dreamer(nn.Module):
     # BPTT through the posterior unroll as ONE cooperative kernel (csrc/pd_rssm_bptt.cu): opt-in with PD_B200_PERSISTENT_BPTT=1.
     # Default is the chain of ~12 launches per timestep: standalone the two take the same 4 ms, but the chain's latency-bound
     # launches share the SMs with the concurrent imagination branch while a cooperative kernel owns all of them for its whole
-    # duration (measured on B200, r02: 27.7 ms/step with the chain, 30.6 ms with the kernel; DESIGN.md).
+    # duration.
     persistent_bptt = os.environ.get("PD_B200_PERSISTENT_BPTT", "0") != "0"
 
     def _persistent_bptt_ok(self, BI):
@@ -829,8 +827,7 @@ class Dreamer(nn.Module):
 
     def _dp_allows(self):
         # Data-parallel runs use the SAME schedule as one GPU (side-stream branches, persistent RSSM kernels, graph replay):
-        # the r02 two-GPU triage matrix (profiles/r02_dp_triage.md) completed in every combination.  PD_B200_DP_FEATURES=0
-        # restores round 1's conservative single-stream / per-timestep-chain schedule under data parallelism.
+        # PD_B200_DP_FEATURES=0 restores a conservative single-stream / per-timestep-chain schedule under data parallelism.
         return self._dp is None or os.environ.get("PD_B200_DP_FEATURES", "1") != "0"
 
     def _side(self, k):
@@ -898,7 +895,7 @@ class Dreamer(nn.Module):
         enc = self.wm.encoder.encoder_image.model
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
-        # ---- encoder (encoders.py:72-96): im2col -> tcgen05 GEMM (+bias+ELU) x4, NHWC activations
+        # ---- encoder (encoders.py:72-96): im2col -> tensor-core GEMM (+bias+ELU) x4, NHWC activations
         img = obs["image"].reshape(NB, IC, 64, 64)
         geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
         embed = b("enc.embed", NB, d.E)
@@ -1528,4 +1525,4 @@ class Dreamer(nn.Module):
 
     def __str__(self):
         n = sum(p.numel() for p in self.parameters())
-        return f"Model: {n} parameters (pydreamer_b200: sm_100a kernels behind the pydreamer Dreamer API)"
+        return f"Model: {n} parameters (pydreamer_b200: sm_90a kernels behind the pydreamer Dreamer API)"

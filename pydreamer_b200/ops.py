@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C ABI (include/pd_b200.h).
 
-`NativeOps` is the product path: every method enqueues one hand-written sm_100a kernel on the
+`NativeOps` is the product path: every method enqueues one hand-written sm_90a kernel on the
 current CUDA stream through libpd_b200.so.  There is no CPU implementation in this package: the
 constructor raises if CUDA or the library is unavailable.
 
@@ -17,7 +17,7 @@ import torch
 from . import _native
 
 ACT_NONE, ACT_ELU = 0, 1
-GEMM_TCGEN05, GEMM_SIMT = 0, 1
+GEMM_TC, GEMM_SIMT = 0, 1
 
 
 _cur_dev = getattr(torch._C, "_cuda_getDevice", None) or torch.cuda.current_device    # the raw binding: no lazy-init checks per launch
@@ -54,19 +54,21 @@ class RssmBwdArgs(ctypes.Structure):
 
 
 class NativeOps:
+    """One library handle on one device.  Its fixed-order gradient reductions use a 16 MB scratch area per stream, for up
+    to eight streams (128 MB of device memory, allocated here); a reduction on a ninth stream raises."""
     is_reference = False
 
     def __init__(self, device):
         device = torch.device(device)
         if device.type != "cuda" or not torch.cuda.is_available():
-            raise RuntimeError("pydreamer_b200 needs a CUDA (sm_100a) device: there is no CPU fallback")
+            raise RuntimeError("pydreamer_b200 needs a CUDA (sm_90a) device: there is no CPU fallback")
         self.device = device
         self.lib = _native.load()
         h = ctypes.c_void_p()
         idx = device.index if device.index is not None else torch.cuda.current_device()
         rc = self.lib.pd_create(int(idx), ctypes.byref(h))
         if rc != 0:
-            raise RuntimeError(f"pd_create failed ({rc}): device {idx} is not an sm_100 GPU or the driver is too old")
+            raise RuntimeError(f"pd_create failed ({rc}): device {idx} is not an sm_90 (H100) GPU or the driver is too old")
         self.h = h
         self._index = int(idx)
         self.gemm_profile = None   # list of (start_event, end_event, flops) when bench.py profiles a step

@@ -12,17 +12,17 @@ os.environ.setdefault("PD_B200_TESTING", "1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA sm_100a device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA sm_90a (H100) device")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu`-marked tests need an sm_100a device: on a box without CUDA a plain `pytest tests` skips them instead of
+    """`gpu`-marked tests need an sm_90a device: on a box without CUDA a plain `pytest tests` skips them instead of
     failing inside torch's CUDA initialisation."""
     import torch
 
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="needs a CUDA sm_100a device (run with -m gpu on the B200 box)")
+    skip = pytest.mark.skip(reason="needs a CUDA sm_90a (H100) device")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

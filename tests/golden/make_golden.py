@@ -1,7 +1,7 @@
-"""Generates tests/golden/*.json from the UNMODIFIED reference (jurgisp/pydreamer @ /root/reference).
+"""Generates tests/golden/*.json from the UNMODIFIED reference (jurgisp/pydreamer).
 
-Run in the authoring container only (the checkout does not exist on the GPU box):
-    python tests/golden/make_golden.py
+Run with a checkout of the reference:
+    python tests/golden/make_golden.py <reference checkout>
 For each case it (1) builds the reference Dreamer, loads seeded weights, (2) seeds the global RNG and runs
 training_step + the four backward passes exactly as train.py:171-187 does, (3) re-draws the same RNG stream as
 explicit noise (SURVEY.md App. D) and checks oracle/dreamer_oracle.py reproduces losses, metrics and gradients,
@@ -14,7 +14,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.abspath(sys.argv[1]))  # a checkout of the reference
 
 from pydreamer.models import Dreamer as RefDreamer  # noqa: E402  (the reference)
 

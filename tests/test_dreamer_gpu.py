@@ -3,7 +3,7 @@ goldens and the oracle.
 
   * exact arm  (SIMT fp32 GEMM, operand rounding off): must reproduce the reference's losses / metrics / gradient
     norms within 2e-4 and the sampled categorical indices bit-exactly;
-  * product arm (tcgen05 TF32 GEMM, rna operand rounding): compared with the oracle TEACHER-FORCED on the indices /
+  * product arm (tensor-core TF32 GEMM, rna operand rounding): compared with the oracle TEACHER-FORCED on the indices /
     actions the GPU run sampled (SURVEY.md §7 'bit-exact categorical indices'): 1e-3 relative on losses, 3e-3 on
     per-tensor gradient norms (north_star tolerance 1e-3 on outputs; gradients of tiny tensors are noisier);
     the number of free-running index flips is reported."""
@@ -122,7 +122,7 @@ def test_optimizer_step_and_second_step_on_gpu():
 
 @pytest.mark.parametrize("case", ("tiny_onehot_log", "tiny_dmc_log", "tiny_iwae3_log"))
 def test_logging_eval_and_inference_branches_on_gpu(case):
-    """do_image_pred + do_dream_tensors, open-loop evaluation and inference() through the native kernels (tcgen05 TF32
+    """do_image_pred + do_dream_tensors, open-loop evaluation and inference() through the native kernels (tensor-core TF32
     product arm) against the reference's committed outputs.  Tolerance 2e-3 (TF32 operands; sums over tensors)."""
     from tests.test_dreamer_cpu import check_log_case, run_log_case
     fx, conf, out = run_log_case(case, DEV)
@@ -185,10 +185,10 @@ def test_full_atari_shape_subbatch_parity_with_oracle(persistent):
 
 @pytest.mark.parametrize("preset", ("atari", "atari_iwae"), ids=("atari", "atari_iwae4_BI200"))
 def test_persistent_rssm_kernel_matches_the_per_step_chain_at_full_size(preset):
-    """pd_rssm_unroll_fwd (one cooperative kernel, fp16 tcgen05 / mma.sync) against the chain of per-timestep launches (TF32
-    tcgen05) on the Atari shape, same weights / batch / noise: both round operands to 10 mantissa bits, so logits agree to
+    """pd_rssm_unroll_fwd (one cooperative kernel, fp16 mma.sync) against the chain of per-timestep launches (TF32
+    tensor-core GEMMs) on the Atari shape, same weights / batch / noise: both round operands to 10 mantissa bits, so logits agree to
     accumulation order and the sampled indices are the same except at numerical near-ties.  `atari_iwae` (B=50 x 4 samples
-    = 200 batch rows) exercises the kernel's batch-row blocks (4 blocks of 64) and strided row owners (200 rows > 148 CTAs)."""
+    = 200 batch rows) exercises the kernel's batch-row blocks (4 blocks of 64) and strided row owners (200 rows > 132 CTAs)."""
     from pydreamer_b200.config import make_conf
     from pydreamer_b200.replay import synthetic_batch
     from oracle.weights import seeded_state_dict
@@ -239,7 +239,7 @@ def test_persistent_rssm_kernel_matches_the_per_step_chain_at_full_size(preset):
                          ids=("atari", "dmc", "atari_iwae4_b16"))
 def test_persistent_bptt_kernel_matches_the_per_step_chain_at_full_size(preset, over):
     """pd_rssm_unroll_bwd (one cooperative kernel: TMA-staged fp16 weight tiles, tf32 mma.sync) against the chain of
-    per-timestep launches (TF32 tcgen05 GEMMs + row-wise kernels) on the SAME forward pass: both contract 10-bit operands,
+    per-timestep launches (TF32 tensor-core GEMMs + row-wise kernels) on the SAME forward pass: both contract 10-bit operands,
     so every tensor the kernel writes agrees with the chain's to accumulation order and weight rounding (fp16 vs tf32
     rounding of the same master weight)."""
     from pydreamer_b200.config import make_conf

@@ -1,7 +1,7 @@
 """GPU parity tests: every hand-written kernel (through the C ABI) against oracle/ref_ops.py on the
 same seeded inputs.  Tolerances are written next to each check:
-  * tcgen05 GEMM with integer-valued operands: bit-exact (tf32 holds them exactly, fp32 sums exact)
-  * tcgen05 GEMM with random fp32 operands:   1e-3 of the output scale (TF32 operand precision)
+  * tensor-core GEMM with integer-valued operands: bit-exact (tf32 holds them exactly, fp32 sums exact)
+  * tensor-core GEMM with random fp32 operands:   1e-3 of the output scale (TF32 operand precision)
   * pointwise / rowwise kernels (operand rounding off): 1e-5 relative
   * categorical sample indices: bit-exact."""
 import pytest
@@ -53,13 +53,13 @@ GEMM_SHAPES = [(128, 128, 32), (128, 128, 256), (50, 1000, 1024), (300, 6144, 10
                (257, 1000, 2048), (2500, 400, 3072), (900, 108, 48),
                # MN-major operands as 3-D TMA boxes: tiles with full 32-column groups followed by groups past the end
                (160, 96, 200),
-               # M in [384, 512): 2-CTA kernel with a quarter of the second 256-row tile past the end
+               # partial last m-tile (the wgmma slices of 16 rows and the mma.sync slices of 32 rows cut at different rows)
                (400, 512, 96), (450, 300, 64),
-               # 2-CTA kernel with K-major operands fetched two 32-wide k-chunks per box: odd chunk count, partial last chunk
+               # odd k-block counts and a partial last k-block
                (1024, 512, 160), (2500, 768, 1000), (1100, 300, 136),
-               # tall with one n-tile: two 128-row tiles per B box (M2 instantiation, M >= 4096)
+               # tall with one n-tile, N below the 128-column tile
                (4500, 48, 48), (5000, 108, 40), (4200, 128, 200),
-               # large enough for the 2-CTA (cta_group::2) 256x256 kernel when PD_GEMM_2CTA=1
+               # many tiles: full waves of persistent CTAs
                (1024, 512, 256), (2500, 6144, 96), (640, 1000, 1000)]
 
 
@@ -111,7 +111,7 @@ def test_gemm_splitk_accumulate_both_mn_major(ops, ref, impl, M, N, K):
 
 @pytest.mark.parametrize("impl", [1, 0])
 def test_gemm_skinny_m_splitk_with_bias_and_residual(ops, ref, impl):
-    """M = 50 rows (one RSSM timestep): the tcgen05 path splits K over the idle SMs; split 0 adds bias+residual."""
+    """M = 50 rows (one RSSM timestep): one row of output tiles over a long K, with bias + residual."""
     ops.set_gemm_impl(impl)
     for (M, N, K, I) in [(50, 1000, 1024, 1), (50, 6144, 2048, 1), (48, 1000, 2048, 4), (50, 2048, 6144, 1)]:
         A, B, bias, res = ints(M, K, seed=1), ints(N, K, seed=2), ints(N, seed=3), ints(M // I, N, seed=4)
@@ -448,21 +448,10 @@ def test_gemm_f16_operands_exact_on_integers(ops, ref, M, N, K):
     close(C, Cr, 1e-6, 1e-6, "f16 strided")
 
 
-def test_gemm_2cta_two_k_chunks_per_box_route(ref):
-    """The opt-in K2 instantiation of the 2-CTA kernel (PD_GEMM_2CTA_K2=1, read when a handle is created): both operands K-major,
-    two 128-byte k-chunks per 3-D TMA box, the stage holding a partial last chunk fetched with 2-D boxes.  Bit-exact."""
-    import os
-    from pydreamer_b200.ops import NativeOps
-    old = os.environ.get("PD_GEMM_2CTA_K2")
-    os.environ["PD_GEMM_2CTA_K2"] = "1"
-    try:
-        o = NativeOps(DEV)
-    finally:
-        if old is None:
-            os.environ.pop("PD_GEMM_2CTA_K2", None)
-        else:
-            os.environ["PD_GEMM_2CTA_K2"] = old
-    o.set_round_operands(False)
+def test_gemm_partial_last_k_block_fp16_and_tf32(ops, ref):
+    """K-major operands (the wgmma path) with odd k-block counts and a partial last k-block, fp16 and tf32.  Bit-exact."""
+    ops.set_gemm_impl(0)
+    o = ops
     for M, N, K in ((2500, 512, 400), (2500, 1000, 2048), (1500, 768, 328), (2500, 6144, 1000)):      # fp16 operands
         A, B = ints(M, K, seed=1), ints(N, K, seed=2)
         bias, res = ints(N, seed=3), ints(M, N, seed=4)
@@ -529,49 +518,35 @@ def test_implicit_conv_gemm_tma_im2col_exact(ops, ref, NB, H, C, k, odim):
     assert torch.equal(C3, C3r), f"mode 3 max diff {(C3 - C3r).abs().max().item()}"
 
 
-@pytest.mark.parametrize("env", [dict(PD_GEMM_CONV_M2="0"), dict(PD_GEMM_CONV_M2="0", PD_GEMM_CONV_2CTA="0"),
-                                 dict(PD_GEMM_CONV_K64="0", PD_GEMM_MN3="0"), dict(PD_GEMM_PLAIN_M2="2")],
-                         ids=["mode1_on_2cta_kernel", "mode1_128x128_tiles", "k32_blocks_2d_boxes", "plain_m2_all_layouts"])
-def test_implicit_conv_gemm_alternative_routes(ref, env):
-    """The routes the default handle does not take (the switches are read when a handle is created): mode 1 on the 2-CTA
-    kernel, mode 1 with plain 128x128 tiles, the K = pixels forms with 32-pixel k-blocks and 2-D boxes.  Bit-exact."""
-    import os
-    from pydreamer_b200.ops import NativeOps
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        o = NativeOps(DEV)
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-    o.set_round_operands(False)
-    for NB, H, C, k, odim in ((9, 30, 48, 6, 96), (21, 14, 96, 4, 192)):
-        P = (H - k) // 2 + 1
-        pixels, K, cpad = NB * P * P, k * k * C, (C + 31) // 32 * 32
-        X = ints(NB, H, H, C, seed=1, lo=-2, hi=3)
-        Wt = ints(K, odim, seed=2, lo=-2, hi=3)
-        dact = ints(pixels, odim, seed=3, lo=-3, hi=3)
-        res = {}
-        for name, oo in (("n", o), ("r", ref)):
-            Cm, db = torch.full((pixels, odim), float("nan"), device=DEV), ints(odim, seed=4).clone()
-            oo.conv_gemm_actbwd(X, k, Wt, Cm, dact, db, o_mn=True)
-            Ot = ints(pixels, odim, seed=5, lo=-2, hi=3)
-            C2, C3 = ints(k * k * cpad, odim, seed=6), ints(odim, k * k * cpad, seed=7)
-            oo.conv_gemm(2, X, k, Ot, C2); oo.conv_gemm(3, X, k, Ot, C3)
-            res[name] = (Cm, db, C2, C3)
-        for a, b_, w in zip(res["n"], res["r"], ("mode 1 + actbwd", "dbias", "mode 2", "mode 3")):
-            assert torch.equal(a, b_), f"{env} {w}: max diff {(a - b_).abs().max().item()}"
-    for M, N, K, b_mn in ((4500, 48, 48, 0), (5000, 108, 40, 1), (4200, 128, 200, 0)):          # tall plain GEMMs (M2 when enabled)
+@pytest.mark.parametrize("NB,H,C,k,odim", [(9, 30, 48, 6, 96), (21, 14, 96, 4, 192), (5, 13, 96, 5, 192), (3, 31, 48, 4, 96)])
+def test_implicit_conv_gemm_all_modes_with_mn_major_weights(ops, ref, NB, H, C, k, odim):
+    """Mode 1 with an MN-major weight plus the fused ELU backward and bias gradient, modes 2 and 3 (K = pixels, split over
+    the SMs), and tall plain GEMMs with one n-tile.  Bit-exact."""
+    ops.set_gemm_impl(0)
+    o = ops
+    P = (H - k) // 2 + 1
+    pixels, K, cpad = NB * P * P, k * k * C, (C + 31) // 32 * 32
+    X = ints(NB, H, H, C, seed=1, lo=-2, hi=3)
+    Wt = ints(K, odim, seed=2, lo=-2, hi=3)
+    dact = ints(pixels, odim, seed=3, lo=-3, hi=3)
+    res = {}
+    for name, oo in (("n", o), ("r", ref)):
+        Cm, db = torch.full((pixels, odim), float("nan"), device=DEV), ints(odim, seed=4).clone()
+        oo.conv_gemm_actbwd(X, k, Wt, Cm, dact, db, o_mn=True)
+        Ot = ints(pixels, odim, seed=5, lo=-2, hi=3)
+        C2, C3 = ints(k * k * cpad, odim, seed=6), ints(odim, k * k * cpad, seed=7)
+        oo.conv_gemm(2, X, k, Ot, C2); oo.conv_gemm(3, X, k, Ot, C3)
+        res[name] = (Cm, db, C2, C3)
+    for a, b_, w in zip(res["n"], res["r"], ("mode 1 + actbwd", "dbias", "mode 2", "mode 3")):
+        assert torch.equal(a, b_), f"{w}: max diff {(a - b_).abs().max().item()}"
+    for M, N, K, b_mn in ((4500, 48, 48, 0), (5000, 108, 40, 1), (4200, 128, 200, 0)):          # tall plain GEMMs
         A = ints(M, K, seed=1)
         B = ints(K, N, seed=2) if b_mn else ints(N, K, seed=2)
         bias = ints(N, seed=3)
         C, Cr = torch.full((M, N), float("nan"), device=DEV), torch.empty(M, N, device=DEV)
         o.gemm(A, B, C, b_mn=bool(b_mn), bias=bias, act=1)
         ref.gemm(A, B, Cr, b_mn=bool(b_mn), bias=bias, act=1)
-        close(C, Cr, 1e-6, 1e-6, f"{env} tall gemm {M, N, K, b_mn}")
+        close(C, Cr, 1e-6, 1e-6, f"tall gemm {M, N, K, b_mn}")
 
 
 @pytest.mark.parametrize("M,N,K,b_mn", [(900, 48, 108, 1), (300, 96, 200, 0), (257, 40, 64, 1), (2500, 192, 96, 1), (130, 18, 40, 0),
@@ -666,3 +641,35 @@ def test_fp16_column_matrix_gemm_store_and_col2im(ops, ref, NB, Hin, k, Cc):
             res[name] = (dec, diff, loss, csum)
         for a, b_, w in zip(res["n"], res["r"], ("dec", "diff", "loss", "csum")):
             close(a, b_, 2e-5, 1e-5, "imgloss over fp16 columns: " + w)
+
+
+def test_gradient_reductions_are_identical_run_to_run(ops):
+    """Bias / LayerNorm / weight gradients summed over many blocks come out bit-identical on every run (fixed summation
+    order, not atomics in arrival order): the training trajectory must not depend on scheduling."""
+    ops.set_gemm_impl(0)
+    g = torch.Generator(device=DEV).manual_seed(5)
+    r = lambda *s: torch.randn(*s, device=DEV, generator=g)
+    x, y = r(40000, 96), r(40000, 96)
+    xs, gamma = r(3000, 400), r(400)
+    mean, rstd = xs.mean(1), xs.var(1, unbiased=False).add(1e-5).rsqrt()
+    A, B = r(2500, 256), r(2500, 384)
+
+    def once():
+        out = dict(colsum=torch.zeros(96, device=DEV), db=torch.zeros(96, device=DEV), dW=torch.zeros(256, 384, device=DEV))
+        ops.colsum(x, out["colsum"])
+        ops.bias_act_bwd(x.clone(), y, 1, out["db"])
+        for rows in (3000, 100):                                   # the many-row and the row-per-block kernels
+            dg, dbt, dbi = (torch.zeros(400, device=DEV) for _ in range(3))
+            ops.ln_elu_bwd(xs[:rows], xs[:rows], xs[:rows].tanh(), gamma, mean[:rows], rstd[:rows],
+                           torch.empty(rows, 400, device=DEV), dg, dbt, dbi)
+            out.update({f"dgamma{rows}": dg, f"dbeta{rows}": dbt, f"dbias{rows}": dbi})
+        ops.gemm(A, B, out["dW"], a_mn=True, b_mn=True, accumulate=True)   # weight gradient: K = 2500 rows
+        torch.cuda.synchronize()
+        return out
+
+    first = once()
+    for _ in range(3):
+        again = once()
+        for k, v in first.items():
+            assert torch.equal(v, again[k]), k
+

@@ -1,4 +1,4 @@
-"""Full-size parity of the PRODUCT arm (tcgen05 TF32 / fp16-forward kernels, persistent RSSM kernels, CUDA-core
+"""Full-size parity of the PRODUCT arm (tensor-core TF32 / fp16-forward kernels, persistent RSSM kernels, CUDA-core
 row-wise kernels — exactly what bench.py times) against the oracle at the BASELINE.json sizes:
 
   config 2  atari       T=B=50, deter 2048, stoch 32x32, H=15            (north_star headline)
@@ -12,11 +12,9 @@ tensor divided by max |g_ref| of the same tensor ("rel-to-max").
 
 Tolerance (north_star: 1e-3 relative).  Losses and metrics (the scalars a training run logs) are held to 1e-3.  Per
 tensor two error measures are printed, dumped (PD_B200_PARITY_DUMP) and asserted:
-  * relative error in the 2-norm, ||x_gpu - x_ref|| / ||x_ref|| <= L2_TOL = 2e-3.  Measured on B200 (profiles/r02_parity_*.json):
-    the large majority of the 113 gradient tensors and 9 of 11 forward tensors of the Atari configuration are inside 1e-3, the
-    worst are reward_rec 1.1e-3, the reward-head gradients 1.7e-3 (they inherit the head's own forward error through the
-    residual), encoder conv-1 weight 1.3e-3, decoder deconv-3 bias 1.5e-3 — every GEMM operand carries 10 mantissa bits
-    (TF32 / fp16, 4.9e-4 per operand, unbiased) through a 50-step recurrence and 4-layer MLPs;
+  * relative error in the 2-norm, ||x_gpu - x_ref|| / ||x_ref|| <= L2_TOL = 2e-3: every GEMM operand carries 10 mantissa
+    bits (TF32 / fp16, 4.9e-4 per operand, unbiased) through a 50-step recurrence and 4-layer MLPs, so a few tensors land
+    above 1e-3 (the run prints each tensor's two errors);
   * worst single element relative to the tensor's largest element <= MAX_TOL = 3e-3.
 Actor and critic gradients are LINEAR in the advantages `agae` (REINFORCE weight, a2c.py:120; critic residual
 value_target - value, a2c.py:103-115), which are differences of O(1) value / reward predictions: at random initialisation
