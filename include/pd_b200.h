@@ -146,8 +146,9 @@ int pd_cat_st_bwd(pd_handle* h, int M, int G, int C, const float* logits, long l
  * buffers the chain of per-step kernels writes (the backward reads them).
  * Caller prepares: hin[0] / zin[0] (masked in_state), x1[0] (pre-norm input of step 0 incl. bias and action term),
  * aa / ea (action and embed projections hoisted over T), fp16 weight copies incl. the TRANSPOSED z_mlp weight ws_wzT16
- * (pd_transpose_to_half).  Limits: BI <= 64, Hd <= 1024, C <= 32, G <= #CTAs, D <= 16 * #CTAs, D and Hd multiples of 8;
- * otherwise PD_ERR_UNSUPPORTED (use the chain). */
+ * (pd_transpose_to_half).  Limits (P = #CTAs = #SMs; KS = 4 when D % 256 == 0, else 1): BI <= 256 and a multiple of I
+ * (rows beyond 64 are taken in blocks of 64), Hd <= 1024, C <= 32, G <= min(P, 256), D <= 16 * P, D and Hd multiples of 8,
+ * ceil(D / (P / KS)) <= 64 and ceil(Hd / (P / KS)) <= 32; otherwise PD_ERR_UNSUPPORTED before any launch (use the chain). */
 typedef struct pd_rssm_fwd_args {
     int T, BI, I, D, Hd, G, C;                 /* rows BI = B*I; Z = G*C; feat row pitch F = D + Z */
     const void *w_z16, *w_ih16, *w_hh16, *w_ph16, *w_pm16;   /* fp16 [Hd,Z] [3D,Hd] [3D,D] [Hd,D] [Z,Hd] */
@@ -183,7 +184,10 @@ int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void* stream);
  * operands of the batched weight-gradient GEMMs, tf32-rounded when round_out != 0.  LayerNorm affine and the two bias
  * gradients fed by LayerNorm inputs are ACCUMULATED (+=) into g_*.  Weights come as TRANSPOSED fp16 copies (pd_transpose_to_half):
  * contraction operands carry 10 mantissa bits on both sides (fp16 weights are exact in tf32; gradients are tf32-rounded fp32),
- * like the TF32 GEMMs of the launch chain this replaces.  Limits: BI <= 64, Hd <= 1024, C <= 32, D/#SMs <= 16. */
+ * like the TF32 GEMMs of the launch chain this replaces.  Limits (P = #CTAs = #SMs; R = min(4, P / G) CTAs per latent
+ * group; ks2 / ks6 = 4 when Z resp. 3D is a multiple of 256, else 1): BI <= min(64, P), ceil(BI / R) <= 16, Hd <= 1024,
+ * C <= 32, G <= P, D <= 16 * P, Hd, D, 3D and Z multiples of 8, ceil(Hd / (P / ks2)) <= 32, ceil(D / (P / ks6)) <= 64,
+ * ceil(Hd / (P / ks6)) <= 32; otherwise PD_ERR_UNSUPPORTED before any launch (use the chain). */
 typedef struct pd_rssm_bwd_args {
     int T, BI, D, Hd, G, C;
     int round_out;

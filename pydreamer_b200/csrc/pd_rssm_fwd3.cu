@@ -33,9 +33,10 @@ typedef Ring<MAXT, 1> RingF;
 typedef Job<MAXT> JobF;
 constexpr int OFF_BAR = RingF::BYTES;
 constexpr int OFF_SH = OFF_BAR + 128;                       // 64 floats: block reductions
-constexpr int OFF_SIDX = OFF_SH + 256;                      // 64 ints: sampled classes of one row
+constexpr int MAXG = 256;                                   // latent groups the kernel takes (phase A keeps one class per group)
+constexpr int OFF_SIDX = OFF_SH + 256;                      // MAXG ints: sampled classes of one row
 constexpr int HB = 256;                                     // batch rows the MULTI instantiation takes (4 blocks of BROWS)
-constexpr int OFF_HC = OFF_SIDX + 256;                      // [16][BROWS or HB] floats: masked h of my units (input of the next step)
+constexpr int OFF_HC = OFF_SIDX + MAXG * 4;                 // [16][BROWS or HB] floats: masked h of my units (input of the next step)
 constexpr int OFF_PART = OFF_HC + 16 * HB * 4;              // [2][1024] floats: phase A gather halves
 constexpr int OFF_LOG = OFF_PART + 2 * 1024 * 4;            // [16 or 64][32] floats: phase D logits of my rows
 constexpr int OFF_GI = OFF_LOG + 64 * 32 * 4;               // [48][65] floats: phase B gi of my units (for the gate math)
@@ -458,7 +459,7 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     // one block of batch rows: the single-block kernel; up to four (IWAE): the MULTI instantiation
     const bool multi = !(a->BI <= BROWS && a->BI <= P && (a->BI + R - 1) / R <= 16);
     const bool ok = a->T >= 1 && a->BI >= 1 && a->BI <= HB && a->I >= 1 && a->BI % a->I == 0 &&
-                    a->Hd <= 4 * NCT && a->Hd % 8 == 0 && a->D % 8 == 0 && a->C >= 1 && a->C <= 32 && a->G >= 1 && a->G <= P &&
+                    a->Hd <= 4 * NCT && a->Hd % 8 == 0 && a->D % 8 == 0 && a->C >= 1 && a->C <= 32 && a->G >= 1 && a->G <= P && a->G <= MAXG &&
                     (a->D + P - 1) / P <= 16 && (a->D + RG - 1) / RG <= 64 &&
                     (a->Hd + RG - 1) / RG <= 32 && Z >= 1 && a->ws_ghpart && a->ws_y2part && a->ws_wzT16;
     if (!ok)

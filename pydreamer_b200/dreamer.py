@@ -816,8 +816,9 @@ class Dreamer(nn.Module):
         ks = 4 if d.D % 256 == 0 and P >= 4 else 1
         R = max(1, min(4, P // d.G))
         cd = lambda a_, b_: -(-a_ // b_)
-        # batch rows (B x iwae_samples) beyond one 64-row MMA operand are taken in blocks by the kernel, up to 256
-        return (BI <= 256 and d.Hd <= 1024 and d.Hd % 8 == 0 and d.D % 8 == 0 and d.C <= 32 and d.G <= P and
+        # batch rows (B x iwae_samples) beyond one 64-row MMA operand are taken in blocks by the kernel, up to 256; at most
+        # 256 latent groups (MAXG of csrc/pd_rssm_fwd3.cu)
+        return (BI <= 256 and d.Hd <= 1024 and d.Hd % 8 == 0 and d.D % 8 == 0 and d.C <= 32 and d.G <= min(P, 256) and
                 cd(d.D, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32 and
                 getattr(self, "_k1_wzT", None) is not None)
 
