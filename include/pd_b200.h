@@ -94,13 +94,14 @@ int pd_conv_gemm(pd_handle* h, int mode, int NB, int H, int W, int C, int k, con
 int pd_to_half(pd_handle* h, long M, long N, const float* src, long lds, void* dst, long ldd, void* stream);
 
 /* ---- LayerNorm(eps, biased var, affine) + ELU -------------------------------------------- */
-/* y = ELU(LN(x)); saves per-row mean / rstd.  common.py:45-51, rssm.py:105,110,115,139-140,144-145. */
+/* y = ELU(LN(x)); saves per-row mean / rstd.  common.py:45-51, rssm.py:105,110,115,139-140,144-145.
+ * 1 <= N <= 1024, otherwise PD_ERR_ARG before any launch. */
 int pd_ln_elu_fwd(pd_handle* h, int M, int N, const float* x, long ldx,
                   const float* gamma, const float* beta, float eps,
                   float* y, long ldy, float* mean, float* rstd,
                   void* y16 /* optional fp16 copy of y (operand of a forward-only pd_gemm_f16) */, long ldy16, void* stream);
-/* dx from dy; ACCUMULATES dgamma, dbeta and (optional) dbias (= column sums of dx, the grad of the
- * bias of the Linear that produced x) with atomics. */
+/* dx from dy; ACCUMULATES (+=) dgamma, dbeta and (optional) dbias (= column sums of dx, the grad of the
+ * bias of the Linear that produced x), summed in a fixed order.  1 <= N <= 1024, otherwise PD_ERR_ARG. */
 int pd_ln_elu_bwd(pd_handle* h, int M, int N, const float* dy, long lddy,
                   const float* x, long ldx, const float* y, long ldy,
                   const float* gamma, const float* mean, const float* rstd,
@@ -122,7 +123,8 @@ int pd_gru_bwd(pd_handle* h, int M, int D, const float* dh_a, long ldda, const f
 
 /* ---- categorical straight-through latent -------------------------------------------------- */
 /* logits[M, G*C] -> per (m,g): l = logits - logsumexp; p = softmax(l); k = argmax_c p_c / q_c
- * (== torch.multinomial's sampling, SURVEY.md App. D); z = onehot(k).  C <= 32.
+ * (== torch.multinomial's sampling, SURVEY.md App. D; exact ties go to the lowest class, torch.argmax's first maximum);
+ * z = onehot(k).  1 <= C <= 32, otherwise PD_ERR_ARG.
  * rssm.py:147-148,178-179,195-201; a2c.py:47-48 with G = 1 for the one-hot actor.
  * zmask (optional) = z * mask_next[m]; idx (optional) int32 [M,G]. */
 int pd_cat_sample(pd_handle* h, int M, int G, int C, const float* logits, long ldl,
@@ -130,7 +132,7 @@ int pd_cat_sample(pd_handle* h, int M, int G, int C, const float* logits, long l
                   float* zmask, long ldzm, const float* mask_next, int32_t* idx,
                   void* z16 /* optional fp16 copy of z */, long ldz16, void* stream);
 /* straight-through backward: dlogits = p * (dz - sum_c p dz) + alpha * rowscale[m] * extra;
- * dz = dz_a + dz_b * mask_b (each optional). */
+ * dz = dz_a + dz_b * mask_b (each optional).  1 <= C <= 32, otherwise PD_ERR_ARG. */
 int pd_cat_st_bwd(pd_handle* h, int M, int G, int C, const float* logits, long ldl,
                   const float* dz_a, long ldda, const float* dz_b, long lddb, const float* mask_b,
                   const float* extra, long ldex, const float* rowscale, float alpha,
@@ -210,8 +212,9 @@ int pd_transpose_to_half(pd_handle* h, int M, int N, const float* src, long lds,
 
 /* ---- KL(post || prior) with balancing, entropies, unweighted grads ------------------------ */
 /* dreamer.py:328-343,369-379.  mode 0 (I == 1): value KL, grads (1-bal)*dKL/dpost and bal*dKL/dprior
- * (bal < 0 => plain KL, kl_balance == 0.5 case dreamer.py:241).  mode 1 (I > 1): sampled
- * log q(z) - log p(z) with idx from pd_cat_sample.  kl_exact / entropies are for metrics. */
+ * (bal < 0 => plain KL, weight 1 on both: the reference's kl_balance 0.5 and 0, dreamer.py:241,334).  mode 1 (I > 1):
+ * sampled log q(z) - log p(z) with idx from pd_cat_sample.  kl_exact / entropies are for metrics.
+ * One block of G warps per row: 1 <= G <= 32 and 1 <= C <= 32, otherwise PD_ERR_ARG. */
 int pd_kl(pd_handle* h, int M, int G, int C, const float* post, long ldpo, const float* prior, long ldpr,
           const int32_t* idx, int mode, float balance,
           float* loss_kl, float* kl_exact, float* ent_post, float* ent_prior,
@@ -304,7 +307,7 @@ int pd_colmean(pd_handle* h, long M, int N, const float* x, float* out, void* st
 /* Column-wise GAE(lambda) scan + reality weights + critic loss/grad.  J = H+1 rows of Md columns.
  * vt = critic_target values, v = critic values, rew = reward head output, term_logit = terminal logits.
  * outputs: adv, agae, target, weight [H,Md]; dv [H,Md] = d loss_critic / d v; term [J,Md] = sigmoid;
- * sums[5] (double) += {loss_critic*HMd, sum v0[0], sum v0, sum r1, sum r1^2}. */
+ * sums[5] (double) += {loss_critic*HMd, sum v0[0], sum v0, sum r1, sum r1^2}.  1 <= H <= 127, otherwise PD_ERR_ARG. */
 int pd_gae_critic(pd_handle* h, int H, int Md, float gamma, float lambda,
                   const float* vt, const float* v, const float* rew, const float* term_logit,
                   float* term, float* adv, float* agae, float* target, float* weight, float* dv,

@@ -27,6 +27,13 @@ from . import ops as _ops
 from .ops import ACT_ELU, ACT_NONE
 
 
+def kl_balance_arg(kl_balance):
+    """The `balance` argument of pd_kl for a configured kl_balance.  The reference (dreamer.py:241,334) maps 0.5 to None
+    and takes the plain KL whenever `not self.kl_balance`, so 0 too means the plain KL (gradient weight 1 on both sides),
+    which pd_kl spells as a negative balance."""
+    return -1.0 if kl_balance in (0.0, 0.5) else float(kl_balance)
+
+
 # ======================================================================================
 # parameter containers (names/shapes identical to the reference's module tree)
 # ======================================================================================
@@ -1035,8 +1042,7 @@ class Dreamer(nn.Module):
         l_kl, kl_exact = b("loss.kl", N), b("loss.klx", N)
         ent_post, ent_prior = b("loss.entq", N), b("loss.entp", N)
         dpost_u, dprior = b("kl.dpost", N, d.Z), b("kl.dprior", N, d.Z)
-        kb = conf.kl_balance
-        ops.kl(post.view(N, d.Z), prior, idx.view(N, d.G), 0 if I == 1 else 1, -1.0 if kb == 0.5 else kb, d.G, d.C,
+        ops.kl(post.view(N, d.Z), prior, idx.view(N, d.G), 0 if I == 1 else 1, kl_balance_arg(conf.kl_balance), d.G, d.C,
                l_kl, kl_exact, ent_post, ent_prior, dpost_u, dprior)
         w, tb = b("loss.w", N), b("loss.tb", NB, 8)
         ops.wm_loss(NB, I, conf.kl_weight, conf.image_weight, conf.reward_weight, conf.terminal_weight, l_img, l_rew,
