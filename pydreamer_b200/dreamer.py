@@ -15,9 +15,9 @@ parameters through a tiny autograd.Function whose backward hands those precomput
 so `loss.backward()` in the caller works unchanged.  Parameters live in one flat arena (views), which
 is what the fused optimizer and the single-bucket data-parallel all-reduce operate on.
 """
-import math
 import contextlib
 import os
+import warnings
 from types import SimpleNamespace
 
 import torch
@@ -32,6 +32,16 @@ def kl_balance_arg(kl_balance):
     and takes the plain KL whenever `not self.kl_balance`, so 0 too means the plain KL (gradient weight 1 on both sides),
     which pd_kl spells as a negative balance."""
     return -1.0 if kl_balance in (0.0, 0.5) else float(kl_balance)
+
+
+def _persistent_sms(m, enabled):
+    """The shared preamble of Dreamer._persistent_rssm_ok / _persistent_bptt_ok: the SM count a persistent RSSM kernel of
+    module `m` spreads over, or None when it cannot run (switched off, restricted under data parallelism, or neither a GPU
+    nor the reference op table, whose stand-ins assume 148 SMs)."""
+    on_gpu = m._arena.is_cuda
+    if not (enabled and m._dp_allows() and (on_gpu or m.ops.is_reference)):
+        return None
+    return torch.cuda.get_device_properties(m._arena.device).multi_processor_count if on_gpu else 148
 
 
 # ======================================================================================
@@ -333,10 +343,16 @@ class Dreamer(nn.Module):
         self.ac = _ActorCritic(features_dim, conf.action_dim, conf.layer_norm, conf.actor_dist)
         self.probe_model = _NoProbeHead()
         # static dims
+        Aout = conf.action_dim if conf.actor_dist == "onehot" else 2 * conf.action_dim
+        cd, IC = conf.cnn_depth, conf.image_channels
         self.d = SimpleNamespace(D=conf.deter_dim, G=conf.stoch_dim, C=conf.stoch_discrete,
                                  Z=conf.stoch_dim * conf.stoch_discrete, Hd=conf.hidden_dim, E=self.wm.encoder.out_dim,
-                                 A=conf.action_dim, F=features_dim, cd=conf.cnn_depth, IC=conf.image_channels,
-                                 Aout=conf.action_dim if conf.actor_dist == "onehot" else 2 * conf.action_dim)
+                                 A=conf.action_dim, F=features_dim, cd=cd, IC=IC, Aout=Aout,
+                                 Ap=(Aout + 3) // 4 * 4)   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
+        # (input size, output size, in channels, out channels) of the four 4x4 stride-2 convolutions of the encoder
+        self._enc_geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
+        # (input size, output size, kernel, in channels, out channels) of the four stride-2 deconvolutions of the decoder
+        self._dec_geo = ((1, 5, 5, 32 * cd, 4 * cd), (5, 13, 5, 4 * cd, 2 * cd), (13, 30, 6, 2 * cd, cd), (30, 64, 6, cd, IC))
         self._arena = None
         self._arena_device = None
         self._ws = {}
@@ -428,7 +444,6 @@ class Dreamer(nn.Module):
         training steps without an optimizer step / zero_grad in between is accumulating gradients in the reference's
         semantics; that is not supported here and is said once instead of silently training on the last micro-batch."""
         if self._grads_pending and not self._warned_accum:
-            import warnings
             warnings.warn("pydreamer_b200: training_step overwrites the gradients of the previous call (groups "
                           f"{sorted(self._grads_pending)} were neither stepped nor zero_grad()-ed): gradient accumulation "
                           "over several training_step calls is not supported")
@@ -491,11 +506,11 @@ class Dreamer(nn.Module):
         if getattr(self, "_test_inference_noise", None) is not None:      # tests pin the sampling noise
             noise = self._test_inference_noise
         feat = self._buf("inf.feat", 1, B, d.F)
-        _, _, _, out_state = self._wm_features(obs, in_state, 1, B, 1, noise, "inf.", feat)
+        out_state = self._wm_features(obs, in_state, 1, B, 1, noise, "inf.", feat).out_state
         f = feat.view(B, d.F)
         alog, val = self._buf("inf.alog", B, d.Aout), self._buf("inf.val", B, 1)
-        self._mlp_fwd(self._mlp_params(self.ac.actor), f, alog, "scratch")
-        self._mlp_fwd(self._mlp_params(self.ac.critic), f, val, "scratch")
+        self._mlp_fwd(self._mlp_params(self.ac.actor), f, alog)
+        self._mlp_fwd(self._mlp_params(self.ac.critic), f, val)
         y = alog.view(1, B, d.Aout).clone()
         if self.conf.actor_dist == "onehot":
             dist = D.OneHotCategorical(logits=y)
@@ -588,55 +603,71 @@ class Dreamer(nn.Module):
         return SimpleNamespace(L=L, lin=[seq[3 * l] for l in range(L)], ln=[seq[3 * l + 1] for l in range(L)],
                                out=seq[3 * L], hid=mlp.hidden_dim, out_dim=mlp.out_dim, in_dim=mlp.in_dim)
 
+    # ------------------------------------------------------------------ dense layers
+    def _fgemm(self, x, w, out, f16, c_zeroed=False, **kw):
+        """out = x·wᵀ (+ the epilogue in kw) with fp16 operands (x in fp16 and the fp16 shadow of w: forward-only layers)
+        or tf32 ones.  c_zeroed (out is pre-cleared for split-K) only concerns the tf32 GEMM."""
+        if f16:
+            self.ops.gemm_f16(x, self._wh(w), out, **kw)
+        else:
+            self.ops.gemm(x, self._w(w), out, c_zeroed=c_zeroed, **kw)
+
+    def _head_fwd(self, layers, h, y, p, m, r, out, f16=False, p16=None, res=None, r_div=1, c_zeroed=False):
+        """out = Linear(LayerNorm+ELU(Linear(h) + res)): the prior or posterior logits of the RSSM (rssm.py:108-116).
+        layers = (Linear, LayerNorm, Linear); y, p, m, r receive the pre-norm input, the ELU output and the LN statistics.
+        f16: fp16 operands, h in fp16 and p16 receiving the fp16 copy of p."""
+        l1, ln, l2 = layers
+        self._fgemm(h, l1.weight, y, f16, bias=self._raw(l1.bias), res=res, r_div=r_div, c_zeroed=c_zeroed)
+        self.ops.ln_elu_fwd(y, self._raw(ln.weight), self._raw(ln.bias), 1e-3, p, m, r, p16)
+        self._fgemm(p16 if f16 else p, l2.weight, out, f16, bias=self._raw(l2.bias), c_zeroed=c_zeroed)
+
     # ------------------------------------------------------------------ MLP forward / backward
-    def _mlp_fwd(self, mp, x_in, out, tag, rows_total=None, row0=0, save=False, x16=None):
-        """out[rows, out_dim] = MLP(x_in).  With save=True the per-layer pre-norm x, post-ELU y and LN
-        statistics are kept in workspace buffers `tag` (rows_total rows, this call fills [row0, row0+rows)).
+    def _mlp_saved(self, mp, tag, rows):
+        """Workspace for what an MLP forward keeps for its backward: per hidden layer the pre-norm x, the post-ELU y and the
+        LayerNorm mean / rstd of `rows` rows (buffers `tag.x0`, `tag.y0`, `tag.m0`, `tag.r0`, ...)."""
+        b = self._buf
+        return SimpleNamespace(x=[b(f"{tag}.x{l}", rows, mp.hid) for l in range(mp.L)],
+                               y=[b(f"{tag}.y{l}", rows, mp.hid) for l in range(mp.L)],
+                               m=[b(f"{tag}.m{l}", rows) for l in range(mp.L)],
+                               r=[b(f"{tag}.r{l}", rows) for l in range(mp.L)])
+
+    def _mlp_fwd(self, mp, x_in, out, saved=None, row0=0, x16=None):
+        """out[rows, out_dim] = MLP(x_in).  With `saved` (from _mlp_saved) the activations the backward needs are kept in
+        its rows [row0, row0+rows); otherwise they go to scratch buffers.
         x16 (optional, fp16 copy of x_in): run the hidden-layer GEMMs with fp16 operands (forward-only use)."""
-        ops = self.ops
+        ops, ns = self.ops, self._scratch_ns
         rows = x_in.shape[0]
-        RT = rows_total or rows
         inp, inp16 = x_in, x16
         f16 = x16 is not None
         for l in range(mp.L):
-            if save:
-                x = self._buf(f"{tag}.x{l}", RT, mp.hid)[row0:row0 + rows]
-                y = self._buf(f"{tag}.y{l}", RT, mp.hid)[row0:row0 + rows]
-                mean = self._buf(f"{tag}.m{l}", RT)[row0:row0 + rows]
-                rstd = self._buf(f"{tag}.r{l}", RT)[row0:row0 + rows]
+            if saved is not None:
+                x, y, mean, rstd = (s[l][row0:row0 + rows] for s in (saved.x, saved.y, saved.m, saved.r))
             else:
-                x = self._buf(f"{self._scratch_ns}mlp.sx", rows, mp.hid)
-                y = self._buf(f"{self._scratch_ns}mlp.sy{l % 2}", rows, mp.hid)
-                mean = self._buf(f"{self._scratch_ns}mlp.sm", rows)
-                rstd = self._buf(f"{self._scratch_ns}mlp.sr", rows)
-            if f16:
-                ops.gemm_f16(inp16, self._wh(mp.lin[l].weight), x, bias=self._raw(mp.lin[l].bias))
-                y16 = self._buf(f"{self._scratch_ns}mlp.h16_{l % 2}", rows, mp.hid, dtype=torch.float16)
-            else:
-                ops.gemm(inp, self._w(mp.lin[l].weight), x, bias=self._raw(mp.lin[l].bias))
-                y16 = None
+                x = self._buf(f"{ns}mlp.sx", rows, mp.hid)
+                y = self._buf(f"{ns}mlp.sy{l % 2}", rows, mp.hid)
+                mean = self._buf(f"{ns}mlp.sm", rows)
+                rstd = self._buf(f"{ns}mlp.sr", rows)
+            y16 = self._buf(f"{ns}mlp.h16_{l % 2}", rows, mp.hid, dtype=torch.float16) if f16 else None
+            self._fgemm(inp16 if f16 else inp, mp.lin[l].weight, x, f16, bias=self._raw(mp.lin[l].bias))
             ops.ln_elu_fwd(x, self._raw(mp.ln[l].weight), self._raw(mp.ln[l].bias), 1e-3, y, mean, rstd, y16)
             inp, inp16 = y, y16
         ops.gemm(inp, self._w(mp.out.weight), out, bias=self._raw(mp.out.bias))     # narrow output layer: fp32 operands
-        return out
 
-    def _mlp_bwd(self, mp, x_in, dout, tag, rows_total=None, din=None, din_accum=False):
-        """Accumulates parameter grads of the MLP; optionally (+)= the input gradient into din."""
+    def _mlp_bwd(self, mp, x_in, dout, saved, din=None, din_accum=False):
+        """Accumulates parameter grads of the MLP from the activations its forward kept in `saved` (first rows of it);
+        optionally (+)= the input gradient into din."""
         ops = self.ops
         rows = x_in.shape[0]
-        RT = rows_total or rows
-        sv = lambda n, l: self._buf(f"{tag}.{n}{l}", RT, mp.hid)[:rows]
-        st = lambda n, l: self._buf(f"{tag}.{n}{l}", RT)[:rows]
+        sv = lambda s, l: s[l][:rows]
         dy = self._buf(f"{self._scratch_ns}mlp.dy", rows, mp.hid)
         dx = self._buf(f"{self._scratch_ns}mlp.dx", rows, mp.hid)
-        ylast = sv("y", mp.L - 1)
-        ops.gemm(dout, ylast, self._g(mp.out.weight), a_mn=True, b_mn=True, accumulate=True)
+        ops.gemm(dout, sv(saved.y, mp.L - 1), self._g(mp.out.weight), a_mn=True, b_mn=True, accumulate=True)
         ops.colsum(dout, self._g(mp.out.bias))
         ops.gemm(dout, self._w(mp.out.weight), dy, b_mn=True)
         for l in reversed(range(mp.L)):
-            ops.ln_elu_bwd(dy, sv("x", l), sv("y", l), self._raw(mp.ln[l].weight), st("m", l), st("r", l), dx,
-                           self._g(mp.ln[l].weight), self._g(mp.ln[l].bias), self._g(mp.lin[l].bias))
-            inp = x_in if l == 0 else sv("y", l - 1)
+            ops.ln_elu_bwd(dy, sv(saved.x, l), sv(saved.y, l), self._raw(mp.ln[l].weight), sv(saved.m, l), sv(saved.r, l),
+                           dx, self._g(mp.ln[l].weight), self._g(mp.ln[l].bias), self._g(mp.lin[l].bias))
+            inp = x_in if l == 0 else sv(saved.y, l - 1)
             ops.gemm(dx, inp, self._g(mp.lin[l].weight), a_mn=True, b_mn=True, accumulate=True)
             if l > 0:
                 ops.gemm(dx, self._w(mp.lin[l].weight), dy, b_mn=True)
@@ -649,10 +680,8 @@ class Dreamer(nn.Module):
         Gaussian noise for the tanh_normal actor."""
         d, dev = self.d, self._arena.device
         post = self._buf("noise.post", T, BI, d.Z).exponential_()
-        if self.conf.actor_dist == "onehot":
-            actor = self._buf("noise.actor", H, N, d.A).exponential_()
-        else:
-            actor = self._buf("noise.actor", H, N, d.A).normal_()
+        actor = self._buf("noise.actor", H, N, d.A)
+        actor = actor.exponential_() if self.conf.actor_dist == "onehot" else actor.normal_()
         prior = self._buf("noise.prior", H, N, d.Z).exponential_()
         out = dict(post=post, actor=actor, prior=prior)
         if image_pred:
@@ -723,20 +752,17 @@ class Dreamer(nn.Module):
             noise = self._draw_noise(T, B * I, N, H, image_pred, dream_log, B)
         if want_grad:
             self.ops.fill(self._garena, 0.0)
-        tm = self._phase_timer
-        if tm is not None:
-            tm.mark("prepare+noise")
+        mark = self._phase_timer.mark if self._phase_timer is not None else (lambda phase: None)
+        mark("prepare+noise")
         par = self._ov(1)
         ac_box = {}
+        feats = self._buf("feats", H + 1, N, self.d.F)     # feats[0] = world-model features, feats[1:] = dream
 
         def run_ac():
-            feats = self._buf("feats", H + 1, N, self.d.F)
-            self._dream(feats, N, H, noise["actor"], noise["prior"], "")
-            if tm is not None:
-                tm.mark("dream")
-            ac_box["out"] = self._actor_critic(feats, N, H, want_grad, "")
-            if tm is not None:
-                tm.mark("actor_critic")
+            dr = self._dream(feats, N, H, noise["actor"], noise["prior"], "")
+            mark("dream")
+            ac_box["out"] = self._actor_critic(feats, dr, N, H, want_grad, "")
+            mark("actor_critic")
 
         def after_features():                       # the dream needs only the (detached) posterior features
             if par:
@@ -747,14 +773,12 @@ class Dreamer(nn.Module):
                 finally:
                     self._scratch_ns = ""
 
-        wm_out = self._wm_forward(obs, in_state, T, B, I, H, noise["post"], open_loop,
-                                  noise["image_pred"] if image_pred else None, after_features=after_features)
-        if tm is not None:
-            tm.mark("wm_forward")
+        wm_out, fw = self._wm_forward(obs, in_state, feats, T, B, I, noise["post"], open_loop,
+                                      noise["image_pred"] if image_pred else None, after_features=after_features)
+        mark("wm_forward")
         if want_grad:
-            self._wm_backward(obs, T, B, I, H)
-        if tm is not None:
-            tm.mark("wm_backward")
+            self._wm_backward(obs, fw)
+        mark("wm_backward")
         if par:
             self._join(1)
             cur = torch.cuda.current_stream(self._arena.device)
@@ -764,7 +788,8 @@ class Dreamer(nn.Module):
             run_ac()
         ac_out = ac_box["out"]
         if dream_log:
-            ac_out["dream_tensors"] = self._dream_for_log(obs, T, B, I, noise["dream_log_actor"], noise["dream_log_prior"])
+            ac_out["dream_tensors"] = self._dream_for_log(obs, feats[0], T, B, I, noise["dream_log_actor"],
+                                                          noise["dream_log_prior"])
         return wm_out, ac_out
 
     _phase_timer = None       # bench.py installs a PhaseTimer (CUDA events between the phases of one eager step)
@@ -799,12 +824,9 @@ class Dreamer(nn.Module):
     persistent_bptt = os.environ.get("PD_B200_PERSISTENT_BPTT", "0") != "0"
 
     def _persistent_bptt_ok(self, BI):
-        d = self.d
-        on_gpu = self._arena.is_cuda
-        if not (self.persistent_bptt and self._dp_allows() and (on_gpu or self.ops.is_reference) and
-                getattr(self, "_k1b_w", None)):
+        d, P = self.d, _persistent_sms(self, self.persistent_bptt and getattr(self, "_k1b_w", None))
+        if P is None:
             return False
-        P = torch.cuda.get_device_properties(self._arena.device).multi_processor_count if on_gpu else 148
         Z = d.G * d.C
         ks2 = 4 if Z % 256 == 0 and P >= 4 else 1
         ks6 = 4 if (3 * d.D) % 256 == 0 and P >= 4 else 1
@@ -816,18 +838,15 @@ class Dreamer(nn.Module):
 
     def _persistent_rssm_ok(self, BI):
         d = self.d
-        on_gpu = self._arena.is_cuda
-        if not (self.persistent_rssm and self.fp16_forward and self._dp_allows() and (on_gpu or self.ops.is_reference)):
+        P = _persistent_sms(self, self.persistent_rssm and self.fp16_forward and getattr(self, "_k1_wzT", None) is not None)
+        if P is None:
             return False
-        P = torch.cuda.get_device_properties(self._arena.device).multi_processor_count if on_gpu else 148
         ks = 4 if d.D % 256 == 0 and P >= 4 else 1
-        R = max(1, min(4, P // d.G))
         cd = lambda a_, b_: -(-a_ // b_)
         # batch rows (B x iwae_samples) beyond one 64-row MMA operand are taken in blocks by the kernel, up to 256; at most
         # 256 latent groups (MAXG of csrc/pd_rssm_fwd3.cu)
         return (BI <= 256 and d.Hd <= 1024 and d.Hd % 8 == 0 and d.D % 8 == 0 and d.C <= 32 and d.G <= min(P, 256) and
-                cd(d.D, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32 and
-                getattr(self, "_k1_wzT", None) is not None)
+                cd(d.D, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32)
 
     def _ov(self, bit):
         # (the eager phase timer of bench.py needs one stream)
@@ -879,7 +898,6 @@ class Dreamer(nn.Module):
                 st["graph"] = g
             except Exception as e:                           # keep running eagerly (same kernels), say so once
                 st["failed"] = True
-                import warnings
                 warnings.warn(f"pydreamer_b200: CUDA graph capture failed ({e}); continuing with eager launches")
                 torch.cuda.synchronize()
                 return self._core(obs, in_state, T, B, I, H, None, True)
@@ -892,41 +910,40 @@ class Dreamer(nn.Module):
         return st["out"]
 
     # ------------------------------------------------------------------ world model forward
+    def _rssm_head(self, prior):
+        """(Linear, LayerNorm, Linear) computing the prior logits (from h) or the posterior ones (from h and the embedding)."""
+        c = self.wm.core.cell
+        return (c.prior_mlp_h, c.prior_norm, c.prior_mlp) if prior else (c.post_mlp_h, c.post_norm, c.post_mlp)
+
     def _wm_features(self, obs, in_state, T, B, I, noise_post, tag, feat, open_loop=False):
-        """Encoder + posterior unroll (forward only).  `feat` (T, B*I, F) receives cat(h, z); every intermediate the
-        backward needs is kept in workspace buffers named `tag + ...`."""
-        ops, d, conf = self.ops, self.d, self.conf
+        """Encoder + posterior unroll (forward only).  `feat` (T, B*I, F) receives cat(h, z).  Returns a namespace of every
+        intermediate the backward reads (workspace buffers named `tag + ...`) and the out_state."""
+        ops, d = self.ops, self.d
         NB, BI = T * B, B * I
-        N = NB * I
-        cd, IC = d.cd, d.IC
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
         enc = self.wm.encoder.encoder_image.model
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
         # ---- encoder (encoders.py:72-96): im2col -> tensor-core GEMM (+bias+ELU) x4, NHWC activations
-        img = obs["image"].reshape(NB, IC, 64, 64)
-        geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
+        img = obs["image"].reshape(NB, d.IC, 64, 64)
         embed = b("enc.embed", NB, d.E)
         ea = b("rssm.ea", NB, d.Hd)
-
-        def encode(r0, r1):                         # images [r0, r1) -> embed rows -> hoisted post_mlp_e product
-            x4 = img[r0:r1].permute(0, 2, 3, 1)
-            for li, (hin_, hout, ci, co) in enumerate(geo):
-                hw = hout * hout
-                act = b(f"enc.a{li}", NB * hw, co)[r0 * hw:r1 * hw]
-                if li > 0 and self.implicit_conv:
-                    ops.conv_gemm(1, x4, 4, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU,
-                                  round_out=True)
-                else:
-                    col = b(f"enc.col{li}", NB * hw, 16 * ci)[r0 * hw:r1 * hw]
-                    ops.im2col(x4, 4, 1 if li == 0 else 0, col, round_out=True)
-                    ops.gemm(col, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
-                x4 = act.view(r1 - r0, hout, hout, co)
-            ops.permute4(x4.view(r1 - r0, 4, 8 * cd, 1), embed[r0:r1].view(r1 - r0, 8 * cd, 4, 1), (0, 2, 1, 3),
-                         round_out=True)                                       # (h,w,c) -> reference (c,h,w) flatten
-            ops.gemm(embed[r0:r1], self._w(cell.post_mlp_e.weight), ea[r0:r1])  # hoisted over T
-
-        encode(0, NB)
+        acts, cols = [], []
+        x4 = img.permute(0, 2, 3, 1)
+        for li, (_, hout, ci, co) in enumerate(self._enc_geo):
+            act, col = b(f"enc.a{li}", NB * hout * hout, co), None
+            if li > 0 and self.implicit_conv:
+                ops.conv_gemm(1, x4, 4, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
+            else:
+                col = b(f"enc.col{li}", NB * hout * hout, 16 * ci)
+                ops.im2col(x4, 4, 1 if li == 0 else 0, col, round_out=True)
+                ops.gemm(col, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
+            acts.append(act)
+            cols.append(col)
+            x4 = act.view(NB, hout, hout, co)
+        ops.permute4(x4.view(NB, 4, 8 * d.cd, 1), embed.view(NB, 8 * d.cd, 4, 1), (0, 2, 1, 3),
+                     round_out=True)                                       # (h,w,c) -> reference (c,h,w) flatten
+        ops.gemm(embed, self._w(cell.post_mlp_e.weight), ea)               # hoisted over T
 
         # ---- RSSM posterior unroll (rssm.py:21-78, 125-153)
         mask = b("rssm.mask", T, BI)
@@ -942,6 +959,9 @@ class Dreamer(nn.Module):
         m2, r2 = b("rssm.m2", T, BI), b("rssm.r2", T, BI)
         post = b("rssm.post", T, BI, d.Z)
         idx = b("rssm.idx", T, BI, d.G, dtype=torch.int32)
+        fw = SimpleNamespace(T=T, B=B, I=I, img=img, embed=embed, enc_act=acts, enc_col=cols, mask=mask, hin=hin, zin=zin,
+                             x1=x1, za=za, m1=m1, r1=r1, gates=gates, y2=y2, pin=pin, m2=m2, r2=r2, post=post, idx=idx)
+        head = self._rssm_head(prior=open_loop)     # open loop (rssm.py:52-53): the "posterior" is the prior, no embed
         W = self._w
         if self._persistent_rssm_ok(BI):
             try:
@@ -949,8 +969,7 @@ class Dreamer(nn.Module):
                 # here because the incoming z need not be one-hot
                 Wh, h16 = self._wh, torch.float16
                 ops.gemm(zin[0], W(cell.z_mlp.weight), x1[0], bias=self._raw(cell.z_mlp.bias), res=aa[:B], r_div=I)
-                ph, pn, pm = ((cell.prior_mlp_h, cell.prior_norm, cell.prior_mlp) if open_loop else
-                              (cell.post_mlp_h, cell.post_norm, cell.post_mlp))
+                ph, pn, pm = head
                 ops.rssm_unroll_fwd(
                     dict(T=T, BI=BI, I=I, D=d.D, Hd=d.Hd, G=d.G, C=d.C), 1e-3,
                     w_z16=Wh(cell.z_mlp.weight), w_ih16=Wh(gru.weight_ih), w_hh16=Wh(gru.weight_hh), w_ph16=Wh(ph.weight),
@@ -963,10 +982,9 @@ class Dreamer(nn.Module):
                     ws_h16=b("k1.h16", BI, d.D, dtype=h16), ws_pin16=b("k1.pin16", BI, d.Hd, dtype=h16),
                     ws_barrier=b("k1.bar", 16, dtype=torch.int32), ws_ghpart=b("k1.ghpart", 4, BI, 3 * d.D),
                     ws_y2part=b("k1.y2part", 4, BI, d.Hd))
-                out_state = (feat[T - 1, :, :d.D].clone(), feat[T - 1, :, d.D:].clone())
-                return img, post, idx, out_state
+                fw.out_state = (feat[T - 1, :, :d.D].clone(), feat[T - 1, :, d.D:].clone())
+                return fw
             except RuntimeError as e:        # e.g. cooperative launch refused (SMs reserved by MPS / green contexts)
-                import warnings
                 warnings.warn(f"pydreamer_b200: persistent RSSM kernel unavailable ({e}); using the per-timestep chain")
                 self.persistent_rssm = False
 
@@ -995,90 +1013,76 @@ class Dreamer(nn.Module):
             if par and not last:                    # h_{t+1} is known: its W_hh product overlaps the posterior MLP
                 with self._fork(2):
                     gh_gemm(t + 1)
-            if not open_loop:
-                ops.gemm(feat[t, :, :d.D], W(cell.post_mlp_h.weight), y2[t], bias=self._raw(cell.post_mlp_h.bias),
-                         res=ea[t * B:(t + 1) * B], r_div=I, c_zeroed=skinny)
-                ops.ln_elu_fwd(y2[t], self._raw(cell.post_norm.weight), self._raw(cell.post_norm.bias), 1e-3, pin[t],
-                               m2[t], r2[t])
-                ops.gemm(pin[t], W(cell.post_mlp.weight), post[t], bias=self._raw(cell.post_mlp.bias), c_zeroed=skinny)
-            else:                                   # open loop (rssm.py:52-53): the "posterior" is the prior, no embed
-                ops.gemm(feat[t, :, :d.D], W(cell.prior_mlp_h.weight), y2[t], bias=self._raw(cell.prior_mlp_h.bias),
-                         c_zeroed=skinny)
-                ops.ln_elu_fwd(y2[t], self._raw(cell.prior_norm.weight), self._raw(cell.prior_norm.bias), 1e-3, pin[t],
-                               m2[t], r2[t])
-                ops.gemm(pin[t], W(cell.prior_mlp.weight), post[t], bias=self._raw(cell.prior_mlp.bias), c_zeroed=skinny)
+            self._head_fwd(head, feat[t, :, :d.D], y2[t], pin[t], m2[t], r2[t], post[t],
+                           res=None if open_loop else ea[t * B:(t + 1) * B], r_div=1 if open_loop else I, c_zeroed=skinny)
             ops.cat_sample(post[t], noise_post[t], d.G, d.C, feat[t, :, d.D:], None if last else zin[t + 1],
                            None if last else mask[t + 1], idx[t])
-        out_state = (feat[T - 1, :, :d.D].clone(), feat[T - 1, :, d.D:].clone())
-        return img, post, idx, out_state
+        fw.out_state = (feat[T - 1, :, :d.D].clone(), feat[T - 1, :, d.D:].clone())
+        return fw
 
-    def _wm_forward(self, obs, in_state, T, B, I, H, noise_post, open_loop=False, noise_image_pred=None,
+    def _wm_forward(self, obs, in_state, feats, T, B, I, noise_post, open_loop=False, noise_image_pred=None,
                     after_features=None):
+        """World-model forward; the posterior features go to feats[0] (N, F).  Returns the losses / metrics / tensors of the
+        step and the namespace of everything _wm_backward reads."""
         ops, d, conf = self.ops, self.d, self.conf
         NB, BI = T * B, B * I
         N = NB * I
-        b, W = self._buf, self._w
-        cell = self.wm.core.cell
-        feats = b("feats", H + 1, N, d.F)            # feats[0] = world-model features, feats[1:] = dream
-        img, post, idx, out_state = self._wm_features(obs, in_state, T, B, I, noise_post, "", feats[0].view(T, BI, d.F),
-                                                      open_loop)
+        b = self._buf
+        fw = self._wm_features(obs, in_state, T, B, I, noise_post, "", feats[0].view(T, BI, d.F), open_loop)
         if after_features is not None:
             after_features()
-        featN = feats[0]                                   # (N, F)
-        hN = featN[:, :d.D]
+        fw.featN = featN = feats[0]                        # (N, F)
         # batched prior (rssm.py:186-193)
-        yp, ppin = b("rssm.yp", N, d.Hd), b("rssm.ppin", N, d.Hd)
-        m3, r3 = b("rssm.m3", N), b("rssm.r3", N)
+        fw.yp, fw.ppin = b("rssm.yp", N, d.Hd), b("rssm.ppin", N, d.Hd)
+        fw.m3, fw.r3 = b("rssm.m3", N), b("rssm.r3", N)
         prior = b("rssm.prior", N, d.Z)
-        ops.gemm(hN, W(cell.prior_mlp_h.weight), yp, bias=self._raw(cell.prior_mlp_h.bias))
-        ops.ln_elu_fwd(yp, self._raw(cell.prior_norm.weight), self._raw(cell.prior_norm.bias), 1e-3, ppin, m3, r3)
-        ops.gemm(ppin, W(cell.prior_mlp.weight), prior, bias=self._raw(cell.prior_mlp.bias))
+        self._head_fwd(self._rssm_head(prior=True), featN[:, :d.D], fw.yp, fw.ppin, fw.m3, fw.r3, prior)
 
         # ---- image decoder + reward / terminal heads on the posterior features
-        dd = self._decode_all(featN, img, obs, N, NB, I, "")
-        image_dec, l_img, l_rew, l_term, rec_r, rec_t = dd["image"], dd["l_img"], dd["l_rew"], dd["l_term"], dd["rec_r"], dd["rec_t"]
+        fw.dec = dd = self._decode_all(featN, fw.img, obs, N, NB, I, "")
 
         # ---- KL + loss assembly (dreamer.py:328-379)
         l_kl, kl_exact = b("loss.kl", N), b("loss.klx", N)
         ent_post, ent_prior = b("loss.entq", N), b("loss.entp", N)
-        dpost_u, dprior = b("kl.dpost", N, d.Z), b("kl.dprior", N, d.Z)
-        ops.kl(post.view(N, d.Z), prior, idx.view(N, d.G), 0 if I == 1 else 1, kl_balance_arg(conf.kl_balance), d.G, d.C,
-               l_kl, kl_exact, ent_post, ent_prior, dpost_u, dprior)
-        w, tb = b("loss.w", N), b("loss.tb", NB, 8)
-        ops.wm_loss(NB, I, conf.kl_weight, conf.image_weight, conf.reward_weight, conf.terminal_weight, l_img, l_rew,
-                    l_term, l_kl, kl_exact, ent_prior, ent_post, w, tb)
+        fw.dpost_u, fw.dprior = b("kl.dpost", N, d.Z), b("kl.dprior", N, d.Z)
+        ops.kl(fw.post.view(N, d.Z), prior, fw.idx.view(N, d.G), 0 if I == 1 else 1, kl_balance_arg(conf.kl_balance), d.G,
+               d.C, l_kl, kl_exact, ent_post, ent_prior, fw.dpost_u, fw.dprior)
+        fw.w, tb = b("loss.w", N), b("loss.tb", NB, 8)
+        ops.wm_loss(NB, I, conf.kl_weight, conf.image_weight, conf.reward_weight, conf.terminal_weight, dd.l_img, dd.l_rew,
+                    dd.l_term, l_kl, kl_exact, ent_prior, ent_post, fw.w, tb)
         means = b("loss.means", 8)
         ops.colmean(tb, means)
         tbv = tb.view(T, B, 8)
         metrics = dict(loss_image=means[1], loss_reward=means[2], loss_terminal=means[3], loss_model=means[0],
                        loss_kl=means[4], entropy_prior=means[5], entropy_post=means[6])
-        sel = (lambda x: x.view(T, B, I, *x.shape[1:])[:, :, 0]) if I == 1 else \
-              (lambda x: x.view(T, B, I, *x.shape[1:]).mean(2))
-        tensors = dict(loss_image=tbv[..., 1], image_rec=sel(image_dec), loss_reward=tbv[..., 2],
-                       reward_rec=sel(rec_r), loss_terminal=tbv[..., 3], terminal_rec=sel(rec_t),
-                       loss_kl=tbv[..., 4], entropy_prior=tbv[..., 5], entropy_post=tbv[..., 6])
+        tensors = dict(loss_image=tbv[..., 1], image_rec=self._sel(dd.image, T, B, I), loss_reward=tbv[..., 2],
+                       reward_rec=self._sel(dd.rec_r, T, B, I), loss_terminal=tbv[..., 3],
+                       terminal_rec=self._sel(dd.rec_t, T, B, I), loss_kl=tbv[..., 4], entropy_prior=tbv[..., 5],
+                       entropy_post=tbv[..., 6])
         if noise_image_pred is not None:
-            self._image_pred(obs, featN, prior, noise_image_pred, T, B, I, metrics, tensors)
-        return dict(loss_model=means[0], out_state=out_state, metrics=metrics, tensors=tensors)
+            self._image_pred(obs, fw, prior, noise_image_pred, metrics, tensors)
+        return dict(loss_model=means[0], out_state=fw.out_state, metrics=metrics, tensors=tensors), fw
 
-    def _image_pred(self, obs, featN, prior, noise, T, B, I, metrics, tensors):
+    @staticmethod
+    def _sel(x, T, B, I):
+        """Per-row values (T*B*I, ...) -> (T, B, ...): the value itself, or with importance samples their mean."""
+        x = x.view(T, B, I, *x.shape[1:])
+        return x[:, :, 0] if I == 1 else x.mean(2)
+
+    def _image_pred(self, obs, fw, prior, noise, metrics, tensors):
         """dreamer.py:383-394: decode from a PRIOR sample (what the model predicts before seeing the observation);
         reports the reconstruction losses as logprob_* and the decoded tensors as *_pred.  Logging branch."""
-        ops, d = self.ops, self.d
-        NB = T * B
-        N = NB * I
-        b = self._buf
+        ops, d, b = self.ops, self.d, self._buf
+        T, B, I = fw.T, fw.B, fw.I
+        NB, N = T * B, T * B * I
         featP = b("p.feat", N, d.F)
-        featP[:, :d.D].copy_(featN[:, :d.D])
+        featP[:, :d.D].copy_(fw.featN[:, :d.D])
         ops.cat_sample(prior, noise, d.G, d.C, featP[:, d.D:])
-        img = obs["image"].reshape(NB, d.IC, 64, 64)
-        dd = self._decode_all(featP, img, obs, N, NB, I, "p.")
+        dd = self._decode_all(featP, fw.img, obs, N, NB, I, "p.")
         zeros = b("p.zeros", N, zero=True)
         w, tb = b("p.loss.w", N), b("p.loss.tb", NB, 8)
-        ops.wm_loss(NB, I, 0.0, 1.0, 1.0, 1.0, dd["l_img"], dd["l_rew"], dd["l_term"], zeros, zeros, zeros, zeros, w, tb)
+        ops.wm_loss(NB, I, 0.0, 1.0, 1.0, 1.0, dd.l_img, dd.l_rew, dd.l_term, zeros, zeros, zeros, zeros, w, tb)
         tbv = tb.view(T, B, 8)
-        sel = (lambda x: x.view(T, B, I, *x.shape[1:])[:, :, 0]) if I == 1 else \
-              (lambda x: x.view(T, B, I, *x.shape[1:]).mean(2))
         lp_img, lp_rew, lp_term = tbv[..., 1], tbv[..., 2], tbv[..., 3]
         nanmean = lambda x: torch.nansum(x) / (~torch.isnan(x)).sum()                # functions.py:150-151
         extra_t = {}
@@ -1090,89 +1094,96 @@ class Dreamer(nn.Module):
         metrics.update(logprob_image=lp_img.mean(), logprob_reward=lp_rew.mean(), logprob_terminal=lp_term.mean(),
                        **{k: nanmean(v) for k, v in extra_t.items()})
         tensors.update(logprob_image=lp_img, logprob_reward=lp_rew, logprob_terminal=lp_term, **extra_t,
-                       image_pred=sel(dd["image"]), reward_pred=sel(dd["rec_r"]), terminal_pred=sel(dd["rec_t"]))
+                       image_pred=self._sel(dd.image, T, B, I), reward_pred=self._sel(dd.rec_r, T, B, I),
+                       terminal_pred=self._sel(dd.rec_t, T, B, I))
 
     def _cols_dtype(self, ncols):
         """Column matrices of the transposed convolutions are written once and read once: fp16 halves that traffic.  The GEMM's
         fp16 TMA store needs 16-byte rows (ncols % 8 == 0); the last layer (k*k*3 columns) stays fp32."""
         return torch.float16 if (self.fp16_forward and self.fp16_cols and ncols % 8 == 0) else torch.float32
 
-    def _decode_all(self, featN, img, obs, N, NB, I, tag):
-        """MultiDecoder.training_step forward (decoders.py:50-108) on features (N,F): image decoder (Linear, then each
-        deconv = GEMM + col2im gather with bias+ELU; the last one fused with the image loss) and the reward / terminal
-        MLP heads with their losses.  Buffers are named `tag + ...` (tag "" = the training pass the backward reads)."""
+    def _image_decoder(self, featN, N, tag, img=None, I=1):
+        """ConvDecoder forward (decoders.py:111-161) on features (N,F): Linear, then each deconvolution as a GEMM into column
+        form + a col2im gather with bias (+ELU).  Given the target images `img` (each the target of I feature rows), the last
+        gather also computes the image loss and its gradient seeds; without, it writes the decoded image."""
         ops, d = self.ops, self.d
-        cd, IC = d.cd, d.IC
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
-        W = self._w
         dec = self.wm.decoder.image.model
-        x0 = b("dec.x0", N, 32 * cd)
-        ops.gemm(featN, W(dec[0].weight), x0, bias=self._raw(dec[0].bias), round_out=True)
-        dgeo = ((1, 5, 5, 32 * cd, 4 * cd), (5, 13, 5, 4 * cd, 2 * cd), (13, 30, 6, 2 * cd, cd), (30, 64, 6, cd, IC))
-        xin = x0
-        for li, (hi, ho, k, ci, co) in enumerate(dgeo):
+        x0 = b("dec.x0", N, 32 * d.cd)
+        ops.gemm(featN, self._w(dec[0].weight), x0, bias=self._raw(dec[0].bias), round_out=True)
+        out = SimpleNamespace(xin=[x0], image=b("dec.image", N, d.IC, 64, 64))     # xin[li]: (rows, ci) input of deconv li
+        for li, (hi, ho, k, ci, co) in enumerate(self._dec_geo):
             cols = b(f"dec.cols{li}", N * hi * hi, k * k * co, dtype=self._cols_dtype(k * k * co))
-            ops.gemm(xin, self._decw[li], cols)
+            ops.gemm(out.xin[li], self._decw[li], cols)
             bias = self._raw(dec[2 + 2 * li].bias)
             if li < 3:
                 a = b(f"dec.d{li}", N, ho, ho, co)
                 ops.col2im(cols, hi, hi, k, bias, ACT_ELU, a, round_out=True)
-                xin = a.view(N * ho * ho, co)
+                out.xin.append(a.view(N * ho * ho, co))
+            elif img is not None:
+                out.diff, out.l_img, out.csum = b("dec.diff", N, d.IC, 64, 64), b("loss.img", N), b("dec.csum", N, d.IC)
+                ops.col2im_imgloss(cols, N, hi, hi, d.IC, k, bias, img, I, out.image, out.diff, out.l_img, out.csum)
             else:
-                image_dec, diff = b("dec.image", N, IC, 64, 64), b("dec.diff", N, IC, 64, 64)
-                l_img, csum = b("loss.img", N), b("dec.csum", N, IC)
-                ops.col2im_imgloss(cols, N, hi, hi, IC, k, bias, img, I, image_dec, diff, l_img, csum)
+                ops.col2im(cols, hi, hi, k, bias, ACT_NONE, out.image.permute(0, 2, 3, 1), round_out=False)
+        return out
+
+    def _decode_all(self, featN, img, obs, N, NB, I, tag):
+        """MultiDecoder.training_step forward (decoders.py:50-108) on features (N,F): the image decoder with its loss and the
+        reward / terminal MLP heads with theirs.  Buffers are named `tag + ...` (tag "" = the training pass the backward
+        reads); returns the image decoder's namespace extended by the heads'."""
+        ops = self.ops
+        b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
+        dd = self._image_decoder(featN, N, tag, img, I)
         # reward / terminal heads (decoders.py:257-319)
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
         yr, yt = b("head.yr", N, 1), b("head.yt", N, 1)
-        self._mlp_fwd(rp, featN, yr, tag + "rew", save=True)
-        self._mlp_fwd(tp, featN, yt, tag + "term", save=True)
-        l_rew, dyr, rec_r = b("loss.rew", N), b("head.dyr", N, 1), b("head.rec_r", N)
-        l_term, dyt, rec_t = b("loss.term", N), b("head.dyt", N, 1), b("head.rec_t", N)
-        ops.scalar_head_loss(0, yr, obs["reward"].reshape(NB), I, l_rew, dyr, rec_r)
-        ops.scalar_head_loss(1, yt, obs["terminal"].reshape(NB), I, l_term, dyt, rec_t)
-        return dict(image=image_dec, l_img=l_img, l_rew=l_rew, l_term=l_term, rec_r=rec_r, rec_t=rec_t)
+        dd.rew, dd.term = self._mlp_saved(rp, tag + "rew", N), self._mlp_saved(tp, tag + "term", N)
+        self._mlp_fwd(rp, featN, yr, dd.rew)
+        self._mlp_fwd(tp, featN, yt, dd.term)
+        dd.l_rew, dd.dyr, dd.rec_r = b("loss.rew", N), b("head.dyr", N, 1), b("head.rec_r", N)
+        dd.l_term, dd.dyt, dd.rec_t = b("loss.term", N), b("head.dyt", N, 1), b("head.rec_t", N)
+        ops.scalar_head_loss(0, yr, obs["reward"].reshape(NB), I, dd.l_rew, dd.dyr, dd.rec_r)
+        ops.scalar_head_loss(1, yt, obs["terminal"].reshape(NB), I, dd.l_term, dd.dyt, dd.rec_t)
+        return dd
 
     # ------------------------------------------------------------------ world model backward
-    def _wm_backward(self, obs, T, B, I, H):
+    def _wm_backward(self, obs, fw):
+        """Gradients of the world-model loss into the arena, from the intermediates `fw` that _wm_forward returned."""
         ops, d, conf = self.ops, self.d, self.conf
+        T, B, I = fw.T, fw.B, fw.I
         NB, BI = T * B, B * I
         N = NB * I
-        cd, IC = d.cd, d.IC
         b, W, G = self._buf, self._w, self._g
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
         enc = self.wm.encoder.encoder_image.model
         dec = self.wm.decoder.image.model
-        featN = b("feats", H + 1, N, d.F)[0]
-        w = b("loss.w", N)
+        featN, w, dd = fw.featN, fw.w, fw.dec
         dfeat = b("bwd.dfeat", N, d.F)
 
         # ---- image decoder backward: seeds = w[n] * image_weight * (dec - target)
-        diff = b("dec.diff", N, IC, 64, 64)
-        csum = b("dec.csum", N, IC)
-        ops.rowscale(diff.view(N, IC * 4096), w, 1, conf.image_weight)
-        ops.rowscale(csum, w, 1, conf.image_weight)
-        ops.colsum(csum, G(dec[8].bias))
-        dgeo = ((1, 5, 5, 32 * cd, 4 * cd), (5, 13, 5, 4 * cd, 2 * cd), (13, 30, 6, 2 * cd, cd), (30, 64, 6, cd, IC))
+        ops.rowscale(dd.diff.view(N, d.IC * 4096), w, 1, conf.image_weight)
+        ops.rowscale(dd.csum, w, 1, conf.image_weight)
+        ops.colsum(dd.csum, G(dec[8].bias))
+        dgeo = self._dec_geo
         impl = [self.implicit_conv and li in (1, 2) for li in range(4)]   # deconv 2,3: 32-channel-aligned NHWC gradients
-        copad = [(dgeo[li][4] + 31) // 32 * 32 for li in range(4)]
-        gdec = [b(f"bwd.gdecwp{li}", dgeo[li][2] ** 2 * copad[li], dgeo[li][3]) if impl[li]
-                else b(f"bwd.gdecw{li}", *self._decw[li].shape) for li in range(4)]
+        copad = [(co + 31) // 32 * 32 if impl[li] else co for li, (_, _, _, _, co) in enumerate(dgeo)]
+        gdec = [b(("bwd.gdecwp" if impl[li] else "bwd.gdecw") + str(li), k * k * copad[li], ci)
+                for li, (_, _, k, ci, _) in enumerate(dgeo)]                 # rows (tap, co padded), as self._decw
         for g_ in gdec:
             ops.fill(g_, 0.0)
         par_w = self._ov(4)                 # weight gradients leave the dfeat -> BPTT critical path (joined at the end)
         side = (lambda: self._fork(4)) if par_w else contextlib.nullcontext
-        dout4 = diff.permute(0, 2, 3, 1)                       # [n,y,x,c] view of the NCHW diff
+        dout4 = dd.diff.permute(0, 2, 3, 1)                    # [n,y,x,c] view of the NCHW diff
         for li in (3, 2, 1, 0):
             hi, ho, k, ci, co = dgeo[li]
-            xin = b("dec.x0", N, 32 * cd) if li == 0 else b(f"dec.d{li - 1}", N, hi, hi, ci).view(N * hi * hi, ci)
+            xin = dd.xin[li]
             dxin = b(f"bwd.dd{li}", N * hi * hi, ci)
             # (li > 0: the ELU backward and the bias gradient of the deconv below ride in the input-gradient GEMM's epilogue)
             below_bias = G(dec[2 * li].bias) if li > 0 else None
             if impl[li]:
                 with side():
-                    ops.conv_gemm(2, dout4, k, xin, gdec[li])                          # weight gradient, rows (tap, co padded)
+                    ops.conv_gemm(2, dout4, k, xin, gdec[li])                          # weight gradient
                 ops.conv_gemm_actbwd(dout4, k, self._decw[li], dxin, xin, below_bias, o_mn=True)   # input gradient
             else:
                 if li == 0:
@@ -1186,50 +1197,41 @@ class Dreamer(nn.Module):
                     ops.gemm_actbwd(dcols, self._decw[li], dxin, xin, below_bias, b_mn=True)
                 else:
                     ops.gemm(dcols, self._decw[li], dxin, b_mn=True, round_out=True)
-            if li > 0:
-                dout4 = dxin.view(N, hi, hi, ci)
-            else:
-                dx0 = dxin
+            dout4 = dxin.view(N, hi, hi, ci)
+        dx0 = dxin
         with side():
             for li, idx_ in enumerate((2, 4, 6, 8)):          # back to ConvTranspose2d layout (Cin,Cout,kh,kw)
                 wt = dec[idx_].weight
                 ci, co, kh, kw = wt.shape
-                src = gdec[li].view(kh, kw, copad[li], ci)[:, :, :co] if impl[li] else gdec[li].view(kh, kw, co, ci)
-                ops.permute4(src, G(wt), (3, 2, 0, 1))
+                ops.permute4(gdec[li].view(kh, kw, copad[li], ci)[:, :, :co], G(wt), (3, 2, 0, 1))
             ops.gemm(dx0, featN, G(dec[0].weight), a_mn=True, b_mn=True, accumulate=True)
             ops.colsum(dx0, G(dec[0].bias))
         ops.gemm(dx0, W(dec[0].weight), dfeat, b_mn=True)                      # first writer of dfeat
 
         # ---- reward / terminal heads
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
-        dyr, dyt = b("head.dyr", N, 1), b("head.dyt", N, 1)
-        ops.rowscale(dyr, w, 1, conf.reward_weight)
-        ops.rowscale(dyt, w, 1, conf.terminal_weight)
-        self._mlp_bwd(rp, featN, dyr, "rew", din=dfeat, din_accum=True)
-        self._mlp_bwd(tp, featN, dyt, "term", din=dfeat, din_accum=True)
+        ops.rowscale(dd.dyr, w, 1, conf.reward_weight)
+        ops.rowscale(dd.dyt, w, 1, conf.terminal_weight)
+        self._mlp_bwd(rp, featN, dd.dyr, dd.rew, din=dfeat, din_accum=True)
+        self._mlp_bwd(tp, featN, dd.dyt, dd.term, din=dfeat, din_accum=True)
 
         # ---- prior branch (batch_prior): dprior = kl_weight * w[n] * dKL/dprior
-        dprior = b("kl.dprior", N, d.Z)
+        dprior = fw.dprior
         ops.rowscale(dprior, w, 1, conf.kl_weight)
-        ppin, yp = b("rssm.ppin", N, d.Hd), b("rssm.yp", N, d.Hd)
         dpp, dyp = b("bwd.dpp", N, d.Hd), b("bwd.dyp", N, d.Hd)
-        ops.gemm(dprior, ppin, G(cell.prior_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
+        ops.gemm(dprior, fw.ppin, G(cell.prior_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
         ops.colsum(dprior, G(cell.prior_mlp.bias))
         ops.gemm(dprior, W(cell.prior_mlp.weight), dpp, b_mn=True)
-        ops.ln_elu_bwd(dpp, yp, ppin, self._raw(cell.prior_norm.weight), b("rssm.m3", N), b("rssm.r3", N), dyp,
+        ops.ln_elu_bwd(dpp, fw.yp, fw.ppin, self._raw(cell.prior_norm.weight), fw.m3, fw.r3, dyp,
                        G(cell.prior_norm.weight), G(cell.prior_norm.bias), G(cell.prior_mlp_h.bias))
         ops.gemm(dyp, featN[:, :d.D], G(cell.prior_mlp_h.weight), a_mn=True, b_mn=True, accumulate=True)
         ops.gemm(dyp, W(cell.prior_mlp_h.weight), dfeat[:, :d.D], b_mn=True, res=dfeat[:, :d.D])
 
         # ---- BPTT through the posterior unroll
         dfeat3 = dfeat.view(T, BI, d.F)
-        mask = b("rssm.mask", T, BI)
-        post, pin, y2 = b("rssm.post", T, BI, d.Z), b("rssm.pin", T, BI, d.Hd), b("rssm.y2", T, BI, d.Hd)
-        m2, r2 = b("rssm.m2", T, BI), b("rssm.r2", T, BI)
-        x1, za = b("rssm.x1", T, BI, d.Hd), b("rssm.za", T, BI, d.Hd)
-        m1, r1 = b("rssm.m1", T, BI), b("rssm.r1", T, BI)
-        gates, hin, zin = b("rssm.gates", T, BI, 4 * d.D), b("rssm.hin", T, BI, d.D), b("rssm.zin", T, BI, d.Z)
-        dpost_u = b("kl.dpost", N, d.Z).view(T, BI, d.Z)
+        mask, post, pin, y2, m2, r2 = fw.mask, fw.post, fw.pin, fw.y2, fw.m2, fw.r2
+        x1, za, m1, r1, gates, hin, zin = fw.x1, fw.za, fw.m1, fw.r1, fw.gates, fw.hin, fw.zin
+        dpost_u = fw.dpost_u.view(T, BI, d.Z)
         w3 = w.view(T, BI)
         dpost = b("bwd.dpost", T, BI, d.Z)
         dy2, dx1 = b("bwd.dy2", T, BI, d.Hd), b("bwd.dx1", T, BI, d.Hd)
@@ -1238,63 +1240,6 @@ class Dreamer(nn.Module):
         dhp, dhc = b("bwd.dhp", T, BI, d.D), b("bwd.dhc", BI, d.D)
         dhin, dzin = b("bwd.dhin", T, BI, d.D), b("bwd.dzin", T, BI, d.Z)
         skinny = BI <= 128
-        # ---- encoder backward (as a function of an image-row range)
-        geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
-        encgw = {}
-
-        def enc_bwd_begin():
-            for li in (1, 2, 3):
-                _, _, ci, co = geo[li]
-                if self.implicit_conv:
-                    encgw[li] = b(f"bwd.gencwp{li}", co, 16 * ((ci + 31) // 32 * 32))   # channels padded to 32 per tap
-                else:
-                    encgw[li] = b(f"bwd.gencw{li}", co, 16 * ci)
-                ops.fill(encgw[li], 0.0)
-
-        def enc_bwd_rows(r0, r1):
-            n = r1 - r0
-            if I == 1:
-                dea_c = dy2.view(N, d.Hd)[r0:r1]
-            else:
-                dea_c = b("bwd.dea_c", NB, d.Hd)[r0:r1]
-                ops.group_sum(dy2.view(N, d.Hd)[r0 * I:r1 * I], I, dea_c)
-            dembed = b("bwd.dembed", NB, d.E)[r0:r1]
-            ops.gemm(dea_c, W(cell.post_mlp_e.weight), dembed, b_mn=True)
-            da = b("bwd.da3", NB * 4, 8 * cd)[r0 * 4:r1 * 4]
-            ops.permute4(dembed.view(n, 8 * cd, 4, 1), da.view(n, 4, 8 * cd, 1), (0, 2, 1, 3))
-            for li in (3, 2, 1, 0):
-                hin_, hout, ci, co = geo[li]
-                hw = hout * hout
-                if li == 3:                 # (layers 2..0: done by the col2im that produced their output gradient)
-                    act = b(f"enc.a{li}", NB * hw, co)[r0 * hw:r1 * hw]
-                    ops.bias_act_bwd(da, act, ACT_ELU, G(enc[2 * li].bias))
-                if li == 0:
-                    col = b(f"enc.col{li}", NB * hw, 16 * ci)[r0 * hw:r1 * hw]
-                    ops.gemm(da, col, G(enc[0].weight).view(co, 16 * ci), a_mn=True, b_mn=True, accumulate=True)
-                    continue
-                if self.implicit_conv:
-                    xprev = b(f"enc.a{li - 1}", NB * hin_ * hin_, ci)[r0 * hin_ * hin_:r1 * hin_ * hin_]
-                    ops.conv_gemm(3, xprev.view(n, hin_, hin_, ci), 4, da, encgw[li])
-                else:
-                    col = b(f"enc.col{li}", NB * hw, 16 * ci)[r0 * hw:r1 * hw]
-                    ops.gemm(da, col, encgw[li], a_mn=True, b_mn=True, accumulate=True)
-                dcol = b(f"bwd.dcol{li}", NB * hw, 16 * ci)[r0 * hw:r1 * hw]
-                ops.gemm(da, self._encw[li], dcol, b_mn=True)
-                da_prev = b(f"bwd.da{li - 1}", NB * hin_ * hin_, ci)[r0 * hin_ * hin_:r1 * hin_ * hin_]
-                act_prev = b(f"enc.a{li - 1}", NB * hin_ * hin_, ci)[r0 * hin_ * hin_:r1 * hin_ * hin_]
-                # fold the column-form gradient back AND go through the ELU / bias of the layer below in the same pass
-                ops.col2im_actbwd(dcol, hout, hout, 4, act_prev, G(enc[2 * (li - 1)].bias), da_prev.view(n, hin_, hin_, ci))
-                da = da_prev
-
-        def enc_bwd_end():
-            for li in (1, 2, 3):
-                _, _, ci, co = geo[li]
-                if self.implicit_conv:
-                    cpad = (ci + 31) // 32 * 32
-                    ops.permute4(encgw[li].view(co, 4, 4, cpad)[..., :ci], G(enc[2 * li].weight), (0, 3, 1, 2))
-                else:
-                    ops.permute4(encgw[li].view(co, 4, 4, ci), G(enc[2 * li].weight), (0, 3, 1, 2))
-
         done = False
         if self._persistent_bptt_ok(BI):
             try:
@@ -1309,7 +1254,6 @@ class Dreamer(nn.Module):
                     ws_part7=b("k1b.part7", 4, BI, d.Hd), ws_barrier=b("k1b.bar", 16, dtype=torch.int32), **self._k1b_w)
                 done = True
             except RuntimeError as e:        # e.g. cooperative launch refused
-                import warnings
                 warnings.warn(f"pydreamer_b200: persistent BPTT kernel unavailable ({e}); using the per-timestep chain")
                 self.persistent_bptt = False
         par = self._ov(2) and not done
@@ -1328,10 +1272,7 @@ class Dreamer(nn.Module):
                 self._join(2)                       # dhin[t + 1]
             ops.gru_bwd(dhp[t], dhin[t + 1] if nxt else None, mask[t + 1] if nxt else None, gates[t], hin[t], dgi[t],
                         dgh[t], dhc)
-            if par:
-                with self._fork(2):
-                    ops.gemm(dgh[t], W(gru.weight_hh), dhin[t], b_mn=True, res=dhc, c_zeroed=skinny)
-            else:
+            with self._fork(2) if par else contextlib.nullcontext():
                 ops.gemm(dgh[t], W(gru.weight_hh), dhin[t], b_mn=True, res=dhc, c_zeroed=skinny)
             ops.gemm(dgi[t], W(gru.weight_ih), dza[t], b_mn=True, c_zeroed=skinny)
             ops.ln_elu_bwd(dza[t], x1[t], za[t], self._raw(cell.in_norm.weight), m1[t], r1[t], dx1[t],
@@ -1354,95 +1295,107 @@ class Dreamer(nn.Module):
         else:
             dea, daa = b("bwd.dea", NB, d.Hd), b("bwd.daa", NB, d.Hd)
             ops.group_sum(f2(dy2), I, dea); ops.group_sum(f2(dx1), I, daa)
-        embed = b("enc.embed", NB, d.E)
-        ops.gemm(dea, embed, G(cell.post_mlp_e.weight), a_mn=True, b_mn=True, accumulate=True)
+        ops.gemm(dea, fw.embed, G(cell.post_mlp_e.weight), a_mn=True, b_mn=True, accumulate=True)
         ops.gemm(daa, obs["action"].reshape(NB, d.A), G(cell.a_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
-        enc_bwd_begin()
-        enc_bwd_rows(0, NB)
-        enc_bwd_end()
+
+        # ---- encoder backward
+        geo = self._enc_geo
+        cpad = [(ci + 31) // 32 * 32 if self.implicit_conv else ci for _, _, ci, _ in geo]   # implicit: 32 channels per tap
+        encgw = {li: b(("bwd.gencwp" if self.implicit_conv else "bwd.gencw") + str(li), geo[li][3], 16 * cpad[li])
+                 for li in (1, 2, 3)}
+        for li in (1, 2, 3):
+            ops.fill(encgw[li], 0.0)
+        if I == 1:
+            dea_c = dy2.view(N, d.Hd)
+        else:
+            dea_c = b("bwd.dea_c", NB, d.Hd)
+            ops.group_sum(dy2.view(N, d.Hd), I, dea_c)
+        dembed = b("bwd.dembed", NB, d.E)
+        ops.gemm(dea_c, W(cell.post_mlp_e.weight), dembed, b_mn=True)
+        da = b("bwd.da3", NB * 4, 8 * d.cd)
+        ops.permute4(dembed.view(NB, 8 * d.cd, 4, 1), da.view(NB, 4, 8 * d.cd, 1), (0, 2, 1, 3))
+        ops.bias_act_bwd(da, fw.enc_act[3], ACT_ELU, G(enc[6].bias))
+        for li in (3, 2, 1):                # (the ELU / bias of layers 2..0: done by the col2im that produced their gradient)
+            hin_, hout, ci, co = geo[li]
+            act_prev = fw.enc_act[li - 1]
+            if self.implicit_conv:
+                ops.conv_gemm(3, act_prev.view(NB, hin_, hin_, ci), 4, da, encgw[li])
+            else:
+                ops.gemm(da, fw.enc_col[li], encgw[li], a_mn=True, b_mn=True, accumulate=True)
+            dcol = b(f"bwd.dcol{li}", NB * hout * hout, 16 * ci)
+            ops.gemm(da, self._encw[li], dcol, b_mn=True)
+            da_prev = b(f"bwd.da{li - 1}", NB * hin_ * hin_, ci)
+            # fold the column-form gradient back AND go through the ELU / bias of the layer below in the same pass
+            ops.col2im_actbwd(dcol, hout, hout, 4, act_prev, G(enc[2 * (li - 1)].bias), da_prev.view(NB, hin_, hin_, ci))
+            da = da_prev
+        ops.gemm(da, fw.enc_col[0], G(enc[0].weight).view(geo[0][3], 16 * geo[0][2]), a_mn=True, b_mn=True, accumulate=True)
+        for li in (1, 2, 3):
+            _, _, ci, co = geo[li]
+            ops.permute4(encgw[li].view(co, 4, 4, cpad[li])[..., :ci], G(enc[2 * li].weight), (0, 3, 1, 2))
         if par_w:
             self._join(4)
 
     # ------------------------------------------------------------------ imagination rollout
     def _dream(self, feats, N, H, noise_actor, noise_prior, tag):
         """dreamer.py:188-216: H x { actor -> sample action -> forward_prior }, forward only (reinforce).
-        feats (H+1, N, F): feats[0] holds the start states; rows 1..H are written here."""
+        feats (H+1, N, F): feats[0] holds the start states; rows 1..H are written here.  Returns what the actor-critic
+        reads: the actor outputs `alog`, its saved activations `actor`, the sampled `actions` and `feats16`, the fp16 copy
+        of feats on the fp16-forward path (else None)."""
         ops, d, conf = self.ops, self.d, self.conf
         b, W = (lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)), self._w
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
         ap = self._mlp_params(self.ac.actor)
-        Ap = (d.Aout + 3) // 4 * 4                   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
-        alog = b("dream.alog", H, N, Ap)[..., :d.Aout]
-        actions = b("dream.actions", H, N, d.A)
+        f16 = self.fp16_forward
+        dr = SimpleNamespace(alog=b("dream.alog", H, N, d.Ap)[..., :d.Aout], actions=b("dream.actions", H, N, d.A),
+                             actor=self._mlp_saved(ap, tag + "actor", H * N),
+                             feats16=b("feats16", H + 1, N, d.F, dtype=torch.float16) if f16 else None)
         aidx = b("dream.aidx", N, 1, dtype=torch.int32)
         aa, x, za = b("dream.aa", N, d.Hd), b("dream.x", N, d.Hd), b("dream.za", N, d.Hd)
         mm, rr = b("dream.m", N), b("dream.r", N)
         gi, gh = b("dream.gi", N, 3 * d.D), b("dream.gh", N, 3 * d.D)
         yp, pp, prior = b("dream.yp", N, d.Hd), b("dream.pp", N, d.Hd), b("dream.prior", N, d.Z)
-        f16 = self.fp16_forward
+        za16, pp16 = (b("dream.za16", N, d.Hd, dtype=torch.float16), b("dream.pp16", N, d.Hd, dtype=torch.float16)) if f16 \
+            else (None, None)
+        fx = dr.feats16 if f16 else feats          # GEMM operand copy of the features
         if f16:
-            f16b = b("feats16", H + 1, N, d.F, dtype=torch.float16)
-            ops.to_half(feats[0], f16b[0])
-            za16, pp16 = b("dream.za16", N, d.Hd, dtype=torch.float16), b("dream.pp16", N, d.Hd, dtype=torch.float16)
-            Wh = self._wh
+            ops.to_half(feats[0], fx[0])
         par = self._ov(2)
-        if f16:
-            gh_gemm = lambda i: ops.gemm_f16(f16b[i][:, :d.D], Wh(gru.weight_hh), gh, bias=self._raw(gru.bias_hh))
-        else:
-            gh_gemm = lambda i: ops.gemm(feats[i][:, :d.D], W(gru.weight_hh), gh, bias=self._raw(gru.bias_hh))
+        gh_gemm = lambda i: self._fgemm(fx[i][:, :d.D], gru.weight_hh, gh, f16, bias=self._raw(gru.bias_hh))
         if par:
             with self._fork(2):
                 gh_gemm(0)
         for i in range(H):
-            f, fn = feats[i], feats[i + 1]
-            fh, fnh = (f16b[i], f16b[i + 1]) if f16 else (None, None)
-            self._mlp_fwd(ap, f, alog[i], tag + "actor", rows_total=H * N, row0=i * N, save=True, x16=fh)
-            if conf.actor_dist == "onehot":
-                ops.cat_sample(alog[i], noise_actor[i], 1, d.A, actions[i], idx=aidx)
-                if d.Hd % 4 == 0:
-                    ops.gather_rows(aidx, self._waT, aa)             # a_mlp(one-hot) = one row of a_mlp^T
-                else:
-                    ops.gemm(actions[i], W(cell.a_mlp.weight), aa)
+            f, fn, xn = feats[i], feats[i + 1], fx[i + 1]
+            self._mlp_fwd(ap, f, dr.alog[i], dr.actor, row0=i * N, x16=fx[i] if f16 else None)
+            onehot = conf.actor_dist == "onehot"
+            if onehot:
+                ops.cat_sample(dr.alog[i], noise_actor[i], 1, d.A, dr.actions[i], idx=aidx)
             else:
-                ops.tanh_normal_sample(alog[i], noise_actor[i], actions[i])
-                ops.gemm(actions[i], W(cell.a_mlp.weight), aa)
-            if f16:
-                ops.gemm_f16(fh[:, d.D:], Wh(cell.z_mlp.weight), x, bias=self._raw(cell.z_mlp.bias), res=aa)
-                ops.ln_elu_fwd(x, self._raw(cell.in_norm.weight), self._raw(cell.in_norm.bias), 1e-3, za, mm, rr, za16)
-                ops.gemm_f16(za16, Wh(gru.weight_ih), gi, bias=self._raw(gru.bias_ih))
-                if par:
-                    self._join(2)
-                else:
-                    gh_gemm(i)
-                ops.gru_fwd(gi, gh, f[:, :d.D], fn[:, :d.D], h16=fnh[:, :d.D])
-                if par and i + 1 < H:               # next step's h·W_hh overlaps prior MLP, sampling and the actor
-                    with self._fork(2):
-                        gh_gemm(i + 1)
-                ops.gemm_f16(fnh[:, :d.D], Wh(cell.prior_mlp_h.weight), yp, bias=self._raw(cell.prior_mlp_h.bias))
-                ops.ln_elu_fwd(yp, self._raw(cell.prior_norm.weight), self._raw(cell.prior_norm.bias), 1e-3, pp, mm, rr, pp16)
-                ops.gemm_f16(pp16, Wh(cell.prior_mlp.weight), prior, bias=self._raw(cell.prior_mlp.bias))
-                ops.cat_sample(prior, noise_prior[i], d.G, d.C, fn[:, d.D:], z16=fnh[:, d.D:])
+                ops.tanh_normal_sample(dr.alog[i], noise_actor[i], dr.actions[i])
+            if onehot and d.Hd % 4 == 0:
+                ops.gather_rows(aidx, self._waT, aa)                 # a_mlp(one-hot) = one row of a_mlp^T
             else:
-                ops.gemm(f[:, d.D:], W(cell.z_mlp.weight), x, bias=self._raw(cell.z_mlp.bias), res=aa)
-                ops.ln_elu_fwd(x, self._raw(cell.in_norm.weight), self._raw(cell.in_norm.bias), 1e-3, za, mm, rr)
-                ops.gemm(za, W(gru.weight_ih), gi, bias=self._raw(gru.bias_ih))
-                if par:
-                    self._join(2)
-                else:
-                    gh_gemm(i)
-                ops.gru_fwd(gi, gh, f[:, :d.D], fn[:, :d.D])
-                if par and i + 1 < H:
-                    with self._fork(2):
-                        gh_gemm(i + 1)
-                ops.gemm(fn[:, :d.D], W(cell.prior_mlp_h.weight), yp, bias=self._raw(cell.prior_mlp_h.bias))
-                ops.ln_elu_fwd(yp, self._raw(cell.prior_norm.weight), self._raw(cell.prior_norm.bias), 1e-3, pp, mm, rr)
-                ops.gemm(pp, W(cell.prior_mlp.weight), prior, bias=self._raw(cell.prior_mlp.bias))
-                ops.cat_sample(prior, noise_prior[i], d.G, d.C, fn[:, d.D:])
+                ops.gemm(dr.actions[i], W(cell.a_mlp.weight), aa)
+            self._fgemm(fx[i][:, d.D:], cell.z_mlp.weight, x, f16, bias=self._raw(cell.z_mlp.bias), res=aa)
+            ops.ln_elu_fwd(x, self._raw(cell.in_norm.weight), self._raw(cell.in_norm.bias), 1e-3, za, mm, rr, za16)
+            self._fgemm(za16 if f16 else za, gru.weight_ih, gi, f16, bias=self._raw(gru.bias_ih))
+            if par:
+                self._join(2)
+            else:
+                gh_gemm(i)
+            ops.gru_fwd(gi, gh, f[:, :d.D], fn[:, :d.D], h16=xn[:, :d.D] if f16 else None)
+            if par and i + 1 < H:               # next step's h·W_hh overlaps prior MLP, sampling and the actor
+                with self._fork(2):
+                    gh_gemm(i + 1)
+            self._head_fwd(self._rssm_head(prior=True), xn[:, :d.D], yp, pp, mm, rr, prior, f16, pp16)
+            ops.cat_sample(prior, noise_prior[i], d.G, d.C, fn[:, d.D:], z16=xn[:, d.D:] if f16 else None)
+        return dr
 
     # ------------------------------------------------------------------ actor critic
-    def _actor_critic(self, feats, N, H, want_grad, tag):
-        """a2c.py:61-149 on the dreamed features (all inputs detached, dreamer.py:153-157)."""
+    def _actor_critic(self, feats, dr, N, H, want_grad, tag):
+        """a2c.py:61-149 on the dreamed features and what _dream returned with them (all inputs detached,
+        dreamer.py:153-157)."""
         ops, d, conf, ac = self.ops, self.d, self.conf, self.ac
         J = H + 1
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
@@ -1451,29 +1404,28 @@ class Dreamer(nn.Module):
         cp, ctp, ap = self._mlp_params(ac.critic), self._mlp_params(ac.critic_target), self._mlp_params(ac.actor)
         rew, tlog = b("ac.rew", J * N, 1), b("ac.tlog", J * N, 1)
         vt, v = b("ac.vt", J * N, 1), b("ac.v", J * N, 1)
-        fall16 = b("feats16", J, N, d.F, dtype=torch.float16).view(J * N, d.F) if self.fp16_forward else None
-        self._mlp_fwd(rp, fall, rew, "scratch", x16=fall16)
-        self._mlp_fwd(tp, fall, tlog, "scratch", x16=fall16)
-        self._mlp_fwd(ctp, fall, vt, "scratch", x16=fall16)
-        self._mlp_fwd(cp, fall, v, tag + "critic", save=True, x16=fall16)
+        fall16 = dr.feats16.view(J * N, d.F) if dr.feats16 is not None else None
+        critic = self._mlp_saved(cp, tag + "critic", J * N)
+        self._mlp_fwd(rp, fall, rew, x16=fall16)
+        self._mlp_fwd(tp, fall, tlog, x16=fall16)
+        self._mlp_fwd(ctp, fall, vt, x16=fall16)
+        self._mlp_fwd(cp, fall, v, critic, x16=fall16)
         term = b("ac.term", J, N)
         adv, agae, target = b("ac.adv", H, N), b("ac.agae", H, N), b("ac.target", H, N)
         weight, dv = b("ac.weight", H, N), b("ac.dv", H * N, 1)
         sums = b("ac.sums", 8, dtype=torch.float64)
         ops.fill(sums.view(torch.float32), 0.0)
         ops.gae_critic(H, N, conf.gamma, conf.lambda_gae, vt, v, rew, tlog, term, adv, agae, target, weight, dv, sums)
-        Ap = (d.Aout + 3) // 4 * 4
-        alog = b("dream.alog", H, N, Ap).view(H * N, Ap)[:, :d.Aout]
-        actions = b("dream.actions", H, N, d.A).view(H * N, d.A)
-        dal = b("ac.dalog", H * N, Ap)[:, :d.Aout]
+        alog, actions = dr.alog.view(H * N, d.Aout), dr.actions.view(H * N, d.A)
+        dal = b("ac.dalog", H * N, d.Ap)[:, :d.Aout]
         if conf.actor_dist == "onehot":
             ops.actor_loss_onehot(conf.entropy, alog, actions, agae, weight, dal, sums[5:7])
         else:
             ops.actor_loss_tanh_normal(conf.entropy, alog, actions, agae, weight, dal, sums[5:7])
         if want_grad:
             fH = fall[:H * N]
-            self._mlp_bwd(cp, fH, dv, tag + "critic", rows_total=J * N)
-            self._mlp_bwd(ap, fH, dal, tag + "actor", rows_total=H * N)
+            self._mlp_bwd(cp, fH, dv, critic)
+            self._mlp_bwd(ap, fH, dal, dr.actor)
         hm = float(H * N)
         s = sums
         r_mean = s[3] / hm
@@ -1487,48 +1439,22 @@ class Dreamer(nn.Module):
                     tensors=dict(value=v.view(J, N), value_target=target, value_advantage=adv,
                                  value_advantage_gae=agae, value_weight=weight))
 
-    def _dream_for_log(self, obs, T, B, I, noise_actor, noise_prior):
-        """dreamer.py:165-180 (do_dream_tensors): dream T-1 steps from the first posterior state of every sequence, decode
-        the imagined images, evaluate the critic (log_only).  Logging branch, no gradients."""
-        ops, d = self.ops, self.d
+    def _dream_for_log(self, obs, featN, T, B, I, noise_actor, noise_prior):
+        """dreamer.py:165-180 (do_dream_tensors): dream T-1 steps from the first posterior state of every sequence (rows of
+        this step's posterior features featN), decode the imagined images, evaluate the critic (log_only).  Logging
+        branch, no gradients."""
+        d = self.d
         Hl, BI = T - 1, B * I
-        N0 = T * B * I
-        feats0 = self._buf("feats", self.imag_horizon + 1, N0, d.F) if ("feats", (self.imag_horizon + 1, N0, d.F), torch.float32) in self._ws \
-            else next(v for k, v in self._ws.items() if k[0] == "feats" and k[1][1] == N0)
         fl = self._buf("dl.feats", Hl + 1, B, d.F)
-        fl[0].copy_(feats0[0][0:BI:I])                                   # states[0, :, 0]
-        self._dream(fl, B, Hl, noise_actor, noise_prior, "dl.")
-        ac = self._actor_critic(fl, B, Hl, False, "dl.")
-        img = self._image_decode(fl.view((Hl + 1) * B, d.F), (Hl + 1) * B, "dl.")
-        actions = self._buf("dl.dream.actions", Hl, B, d.A)
+        fl[0].copy_(featN[0:BI:I])                                       # states[0, :, 0]
+        dr = self._dream(fl, B, Hl, noise_actor, noise_prior, "dl.")
+        ac = self._actor_critic(fl, dr, B, Hl, False, "dl.")
+        img = self._image_decoder(fl.view((Hl + 1) * B, d.F), (Hl + 1) * B, "dl.").image
         t = ac["tensors"]
-        return dict(action_pred=torch.cat([obs["action"][:1], actions]), reward_pred=ac["rew"], terminal_pred=ac["term"],
+        return dict(action_pred=torch.cat([obs["action"][:1], dr.actions]), reward_pred=ac["rew"], terminal_pred=ac["term"],
                     image_pred=img.view(T, B, d.IC, 64, 64), value=t["value"], value_target=t["value_target"],
                     value_advantage=t["value_advantage"], value_advantage_gae=t["value_advantage_gae"],
                     value_weight=t["value_weight"])
-
-    def _image_decode(self, featN, N, tag):
-        """ConvDecoder.forward (decoders.py:157-161) without a loss: (N,F) -> (N,C,64,64)."""
-        ops, d = self.ops, self.d
-        cd, IC = d.cd, d.IC
-        b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
-        dec = self.wm.decoder.image.model
-        x0 = b("dec.x0", N, 32 * cd)
-        ops.gemm(featN, self._w(dec[0].weight), x0, bias=self._raw(dec[0].bias), round_out=True)
-        dgeo = ((1, 5, 5, 32 * cd, 4 * cd), (5, 13, 5, 4 * cd, 2 * cd), (13, 30, 6, 2 * cd, cd), (30, 64, 6, cd, IC))
-        xin = x0
-        for li, (hi, ho, k, ci, co) in enumerate(dgeo):
-            cols = b(f"dec.cols{li}", N * hi * hi, k * k * co, dtype=self._cols_dtype(k * k * co))
-            ops.gemm(xin, self._decw[li], cols)
-            bias = self._raw(dec[2 + 2 * li].bias)
-            if li < 3:
-                a = b(f"dec.d{li}", N, ho, ho, co)
-                ops.col2im(cols, hi, hi, k, bias, ACT_ELU, a, round_out=True)
-                xin = a.view(N * ho * ho, co)
-            else:
-                out = b("dec.image", N, IC, 64, 64)
-                ops.col2im(cols, hi, hi, k, bias, ACT_NONE, out.permute(0, 2, 3, 1), round_out=False)
-        return out
 
     def __str__(self):
         n = sum(p.numel() for p in self.parameters())

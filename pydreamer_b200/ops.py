@@ -71,7 +71,7 @@ class NativeOps:
             raise RuntimeError(f"pd_create failed ({rc}): device {idx} is not an sm_90 (H100) GPU or the driver is too old")
         self.h = h
         self._index = int(idx)
-        self.gemm_profile = None   # list of (start_event, end_event, flops) when bench.py profiles a step
+        self.gemm_profile = None   # list of (start_event, end_event, flops, shape key) when bench.py profiles a step
 
     def __del__(self):
         try:
@@ -101,6 +101,18 @@ class NativeOps:
     def launch_count(self):
         return int(self.lib.pd_launch_count(self.h))
 
+    def _profiled(self, launch, flops, shape):
+        """Runs launch().  While bench.py profiles a step (gemm_profile is a list), the launch is bracketed by CUDA events
+        and (start_event, end_event, flops, shape key) is appended to gemm_profile."""
+        prof = self.gemm_profile
+        if prof is None:
+            return launch()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        launch()
+        e1.record()
+        prof.append((e0, e1, flops, shape))
+
     # ------------------------------------------------------------------ gemm
     def gemm(self, A, B, C, *, a_mn=False, b_mn=False, bias=None, res=None, r_div=1, act=ACT_NONE,
              round_out=False, accumulate=False, c_zeroed=False):
@@ -109,18 +121,11 @@ class NativeOps:
         K = A.shape[0] if a_mn else A.shape[1]
         assert (A.shape[1] if a_mn else A.shape[0]) == M, (A.shape, C.shape, a_mn)
         assert (B.shape == (K, N)) if b_mn else (B.shape == (N, K)), (B.shape, (N, K), b_mn)
-        prof = self.gemm_profile
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
         flags = (1 if c_zeroed else 0) | (2 if C.dtype == torch.float16 else 0)       # PD_GEMM_C_ZEROED | PD_GEMM_C_F16
-        rc = self.lib.pd_gemm(self.h, M, N, K, _ptr(A), _ld(A), int(a_mn), _ptr(B), _ld(B), int(b_mn),
-                              _ptr(C), _ld(C), _ptr(bias), _ptr(res), _ld(res) if res is not None else 0,
-                              int(r_div), int(act), int(round_out), int(accumulate), flags, self._s())
-        self._ck(rc, "pd_gemm")
-        if prof is not None:
-            e1.record()
-            prof.append((e0, e1, 2.0 * M * N * K, (M, N, K, int(a_mn), int(b_mn), int(accumulate))))
+        self._profiled(lambda: self._ck(self.lib.pd_gemm(
+            self.h, M, N, K, _ptr(A), _ld(A), int(a_mn), _ptr(B), _ld(B), int(b_mn), _ptr(C), _ld(C), _ptr(bias), _ptr(res),
+            _ld(res) if res is not None else 0, int(r_div), int(act), int(round_out), int(accumulate), flags, self._s()),
+            "pd_gemm"), 2.0 * M * N * K, (M, N, K, int(a_mn), int(b_mn), int(accumulate)))
         return C
 
     def gemm_f16(self, A16, B16, C, *, bias=None, res=None, r_div=1, act=ACT_NONE, round_out=False):
@@ -128,17 +133,10 @@ class NativeOps:
         M, N = C.shape
         K = A16.shape[1]
         assert A16.dtype == torch.float16 and B16.dtype == torch.float16 and B16.shape == (N, K) and A16.shape[0] == M
-        prof = self.gemm_profile
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        rc = self.lib.pd_gemm_f16(self.h, M, N, K, _ptr(A16), _ld(A16), _ptr(B16), _ld(B16), _ptr(C), _ld(C), _ptr(bias),
-                                  _ptr(res), _ld(res) if res is not None else 0, int(r_div), int(act), int(round_out),
-                                  self._s())
-        self._ck(rc, "pd_gemm_f16")
-        if prof is not None:
-            e1.record()
-            prof.append((e0, e1, 2.0 * M * N * K, (M, N, K, "f16", 0, 0)))
+        self._profiled(lambda: self._ck(self.lib.pd_gemm_f16(
+            self.h, M, N, K, _ptr(A16), _ld(A16), _ptr(B16), _ld(B16), _ptr(C), _ld(C), _ptr(bias), _ptr(res),
+            _ld(res) if res is not None else 0, int(r_div), int(act), int(round_out), self._s()), "pd_gemm_f16"),
+            2.0 * M * N * K, (M, N, K, "f16", 0, 0))
         return C
 
     def conv_gemm(self, mode, X, k, O, Cmat, *, o_mn=False, bias=None, act=ACT_NONE, round_out=False):
@@ -146,17 +144,11 @@ class NativeOps:
         NB, H, W, C = X.shape
         assert X.is_contiguous()
         odim = Cmat.shape[1] if mode in (1, 2) else Cmat.shape[0]
-        prof = self.gemm_profile
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        self._ck(self.lib.pd_conv_gemm(self.h, int(mode), NB, H, W, C, int(k), _ptr(X), _ptr(O), _ld(O), int(o_mn), odim,
-                                       _ptr(Cmat), _ld(Cmat), _ptr(bias), int(act), int(round_out), 0 if mode == 1 else 1,
-                                       self._s()), "pd_conv_gemm")
-        if prof is not None:
-            e1.record()
-            P, Q = (H - k) // 2 + 1, (W - k) // 2 + 1
-            prof.append((e0, e1, 2.0 * NB * P * Q * k * k * C * odim, (NB * P * Q, odim, k * k * C, f"conv{mode}", int(o_mn), 0)))
+        P, Q = (H - k) // 2 + 1, (W - k) // 2 + 1
+        self._profiled(lambda: self._ck(self.lib.pd_conv_gemm(
+            self.h, int(mode), NB, H, W, C, int(k), _ptr(X), _ptr(O), _ld(O), int(o_mn), odim, _ptr(Cmat), _ld(Cmat),
+            _ptr(bias), int(act), int(round_out), 0 if mode == 1 else 1, self._s()), "pd_conv_gemm"),
+            2.0 * NB * P * Q * k * k * C * odim, (NB * P * Q, odim, k * k * C, f"conv{mode}", int(o_mn), 0))
         return Cmat
 
     def to_half(self, src, dst):
@@ -278,15 +270,9 @@ class NativeOps:
         """C = (A B^T) * elu'(dact); dbias += column sums (pd_gemm_actbwd: GEMM + bias_act_bwd in one launch)."""
         M, N = C.shape
         K = A.shape[0] if a_mn else A.shape[1]
-        prof = self.gemm_profile
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        self._ck(self.lib.pd_gemm_actbwd(self.h, M, N, K, _ptr(A), _ld(A), int(a_mn), _ptr(B), _ld(B), int(b_mn), _ptr(C), _ld(C),
-                                         _ptr(dact), _ld(dact), _ptr(dbias), self._s()), "pd_gemm_actbwd")
-        if prof is not None:
-            e1.record()
-            prof.append((e0, e1, 2.0 * M * N * K, (M, N, K, int(a_mn), int(b_mn), 0)))
+        self._profiled(lambda: self._ck(self.lib.pd_gemm_actbwd(
+            self.h, M, N, K, _ptr(A), _ld(A), int(a_mn), _ptr(B), _ld(B), int(b_mn), _ptr(C), _ld(C), _ptr(dact), _ld(dact),
+            _ptr(dbias), self._s()), "pd_gemm_actbwd"), 2.0 * M * N * K, (M, N, K, int(a_mn), int(b_mn), 0))
         return C
 
     def conv_gemm_actbwd(self, X, k, O, Cmat, dact, dbias, *, o_mn=False):
@@ -294,16 +280,11 @@ class NativeOps:
         NB, H, W, C = X.shape
         assert X.is_contiguous()
         odim = Cmat.shape[1]
-        prof = self.gemm_profile
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        self._ck(self.lib.pd_conv_gemm_actbwd(self.h, NB, H, W, C, int(k), _ptr(X), _ptr(O), _ld(O), int(o_mn), odim, _ptr(Cmat),
-                                              _ld(Cmat), _ptr(dact), _ld(dact), _ptr(dbias), self._s()), "pd_conv_gemm_actbwd")
-        if prof is not None:
-            e1.record()
-            P, Q = (H - k) // 2 + 1, (W - k) // 2 + 1
-            prof.append((e0, e1, 2.0 * NB * P * Q * k * k * C * odim, (NB * P * Q, odim, k * k * C, "conv1", int(o_mn), 0)))
+        P, Q = (H - k) // 2 + 1, (W - k) // 2 + 1
+        self._profiled(lambda: self._ck(self.lib.pd_conv_gemm_actbwd(
+            self.h, NB, H, W, C, int(k), _ptr(X), _ptr(O), _ld(O), int(o_mn), odim, _ptr(Cmat), _ld(Cmat), _ptr(dact),
+            _ld(dact), _ptr(dbias), self._s()), "pd_conv_gemm_actbwd"),
+            2.0 * NB * P * Q * k * k * C * odim, (NB * P * Q, odim, k * k * C, "conv1", int(o_mn), 0))
         return Cmat
 
     def col2im_actbwd(self, col, Hin, Win, k, dact, dbias, out):

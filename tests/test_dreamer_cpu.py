@@ -256,3 +256,29 @@ def check_log_case(fx, conf, out, rtol):
 def test_logging_eval_and_inference_branches_match_reference(ref_ops, case):
     fx, conf, out = run_log_case(case)
     check_log_case(fx, conf, out, 3e-4)
+
+
+def test_dream_tensors_start_from_the_same_calls_posterior(ref_ops):
+    """do_dream_tensors dreams from the posterior features of its own call, also when that call's imag_horizon differs from
+    an earlier call's: a model that already ran a step on other observations returns the dream tensors of a fresh one."""
+    fx, conf, obs_b, state, _ = build_case("tiny_onehot")
+    obs_a = {k: v.flip(0) if v.is_floating_point() else v for k, v in obs_b.items()}
+    H = conf.imag_horizon
+
+    def model():
+        m = Dreamer(conf)
+        m.load_state_dict(seeded_weights(m.state_dict(), fx))
+        return m
+
+    def dream(m, obs, seed, **kw):
+        torch.manual_seed(seed)
+        return m.training_step(obs, state, **kw)[4]
+
+    a, b = model(), model()
+    with torch.no_grad():
+        dream(a, obs_a, 1)
+        got = dream(a, obs_b, 2, imag_horizon=H - 1, do_dream_tensors=True)
+        want = dream(b, obs_b, 2, imag_horizon=H - 1, do_dream_tensors=True)
+    assert set(got) == set(want) and "value_target" in got
+    for k in want:
+        assert torch.equal(got[k], want[k]), (k, float((got[k] - want[k]).abs().max()))
