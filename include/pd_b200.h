@@ -39,7 +39,7 @@ typedef struct pd_handle pd_handle;
 #define PD_GEMM_TC 0      /* TMA-fed tensor-core (mma.sync tf32 / fp16) kernel (default, the product path) */
 #define PD_GEMM_SIMT 1    /* plain fp32 CUDA-core tile kernel: validation arm for the tests  */
 #define PD_GEMM_C_ZEROED 1 /* pd_gemm flags bit */
-#define PD_GEMM_C_F16 2    /* pd_gemm flags bit: C is an fp16 matrix (ldc in halfs); not with accumulate */
+#define PD_GEMM_C_F16 2    /* pd_gemm flags bit: C is an fp16 matrix (ldc in halfs); not with accumulate / residual */
 
 /* ---- lifetime ---------------------------------------------------------------------------- */
 /* A handle allocates 8 scratch areas of 16 MB on its device for the fixed-order gradient reductions, one per stream it
@@ -62,9 +62,11 @@ int pd_set_round_operands(pd_handle* h, int on);
  *   accumulate = 1: adds into C (split-K partials are summed in a fixed order; bias/R/act must be off).
  * Replaces every nn.Linear / nn.GRUCell matmul and the conv/deconv contractions:
  * common.py:47-55, rssm.py:103-116,138-146, rnn.py:60-67, encoders.py:80-90, decoders.py:128-155.
+ * round_out rounds C to tf32 only while pd_set_round_operands is on (as every producer of this ABI does).
  * flags: PD_GEMM_C_ZEROED = the caller has already cleared C (accepted; the kernel never needs to clear C itself);
  *        PD_GEMM_C_F16 = C points to an fp16 matrix (the deconvolution column matrices of the decoder forward: they are
- *        written once and read once, in fp16 they cost half the HBM traffic; decoders.py:149-155).
+ *        written once and read once, in fp16 they cost half the HBM traffic; decoders.py:149-155); not with accumulate
+ *        or a residual (PD_ERR_ARG).
  * TMA constraints (tensor-core impl): lda/ldb multiples of 4 elements, base pointers 16-byte aligned. */
 int pd_gemm(pd_handle* h, int M, int N, int K,
             const float* A, long lda, int a_mn,

@@ -102,15 +102,15 @@ int pd_gemm(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_m
     PD_REQUIRE(h, !(accumulate && (bias || R || act)), "pd_gemm: accumulate excludes bias/residual/act");
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
-    e.act = act; e.round_out = round_out; e.accumulate = accumulate;
+    e.act = act; e.round_out = round_out && h->round_ops; e.accumulate = accumulate;
     e.c_f16 = (flags & PD_GEMM_C_F16) ? 1 : 0;
     e.dact = nullptr; e.lddact = 0;
-    PD_REQUIRE(h, !(e.c_f16 && accumulate), "pd_gemm: an fp16 output cannot accumulate");
+    PD_REQUIRE(h, !(e.c_f16 && (accumulate || R)), "pd_gemm: an fp16 output cannot accumulate or add a residual");
     // Skinny / unaligned contractions (scalar heads N=1, action inputs K=18, ...) cannot be described
     // by a TMA tensor map (16-byte strides) and have no tensor-core work to speak of: CUDA cores.
     const bool tma_ok = (lda % 4 == 0) && (ldb % 4 == 0) && ((((uintptr_t)A) & 15) == 0) &&
                         ((((uintptr_t)B) & 15) == 0) && N >= 8 && K >= 8 &&
-                        (!e.c_f16 || ((ldc % 8 == 0) && !R && !round_out && ((((uintptr_t)C) & 15) == 0)));
+                        (!e.c_f16 || ((ldc % 8 == 0) && !e.round_out && ((((uintptr_t)C) & 15) == 0)));
     if (h->gemm_impl == PD_GEMM_SIMT || !tma_ok)
         return pd_gemm_simt_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream);
     return pd_gemm_tc_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
@@ -123,7 +123,7 @@ int pd_conv_gemm(pd_handle* h, int mode, int NB, int H, int W, int C, int k, con
     PD_REQUIRE(h, (mode == 1) == (accumulate == 0), "pd_conv_gemm: mode 1 stores, modes 2/3 accumulate");
     PdEpilogue e;
     e.C = Cmat; e.ldc = ldc; e.bias = bias; e.R = nullptr; e.ldr = 0; e.r_div = 1;
-    e.act = act; e.round_out = round_out; e.accumulate = accumulate; e.c_f16 = 0;
+    e.act = act; e.round_out = round_out && h->round_ops; e.accumulate = accumulate; e.c_f16 = 0;
     e.dact = nullptr; e.lddact = 0;
     return pd_conv_gemm_launch(h, mode, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
 }
@@ -135,7 +135,7 @@ int pd_gemm_f16(pd_handle* h, int M, int N, int K, const void* A, long lda, cons
     PD_REQUIRE(h, A && B && C, "pd_gemm_f16: null operand");
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
-    e.act = act; e.round_out = round_out; e.accumulate = 0; e.c_f16 = 0;
+    e.act = act; e.round_out = round_out && h->round_ops; e.accumulate = 0; e.c_f16 = 0;
     e.dact = nullptr; e.lddact = 0;
     return pd_gemm_tc_launch(h, M, N, K, A, lda, 0, B, ldb, 0, e, (cudaStream_t)stream, 1);
 }

@@ -25,7 +25,6 @@ non-zero values, so `+=` and `=` differ.
 PD_TEST_DEV=cpu runs the file with the float32 torch twins of oracle/ref_ops.py in place of the kernels: a dry run of the
 references and bounds without a GPU."""
 import math
-import os
 
 import pytest
 import torch
@@ -33,11 +32,9 @@ import torch.distributions as D
 import torch.nn.functional as F
 
 from oracle.ref_ops import RefOps
+from tests.util import CPU, DEV, Gen, bound, f64, fp16, fp32, ops, round_out, rounded, ulp  # noqa: F401
 
-DEV = os.environ.get("PD_TEST_DEV", "cuda:0")
-CPU = DEV == "cpu"
 gpu = pytest.mark.gpu if not CPU else (lambda f: f)
-f64 = torch.float64
 U = 2.0 ** -24                                  # unit roundoff of fp32
 ELU_REL = 5e-7                                  # relative error of pd_elu's ex2.approx branch (pd_common.cuh:104-125)
 TINY = 2.0 ** -126                              # fp32 underflow: anything below this may flush or lose bits
@@ -47,90 +44,7 @@ IDX_GUARD = -777
 NAN = float("nan")
 
 
-@pytest.fixture(scope="module")
-def ops(request):
-    if CPU:
-        yield RefOps("cpu")
-        return
-    o = request.getfixturevalue("native_ops")
-    yield o
-    o.set_round_operands(True)
-    o.set_gemm_impl(0)
-
-
-@pytest.fixture(params=[0, 1], ids=lambda v: f"round_out{v}")
-def round_out(request, ops):
-    ops.set_round_operands(bool(request.param))
-    yield request.param
-    ops.set_round_operands(True)
-
-
 # ----------------------------------------------------------------------------------------------------- helpers
-# Gen, fp32, fp16, ulp, tf32_rna, bound and rounded are those of tests/test_rssm_persistent_gpu.py.
-class Gen:
-    def __init__(self, seed):
-        self.g = torch.Generator().manual_seed(seed)
-
-    def uniform(self, *shape, bound=1.0):
-        return ((torch.rand(*shape, generator=self.g, dtype=f64) * 2 - 1) * bound).to(DEV)
-
-    def normal(self, *shape, scale=1.0):
-        return (torch.randn(*shape, generator=self.g, dtype=f64) * scale).to(DEV)
-
-    def rand(self, *shape):
-        return torch.rand(*shape, generator=self.g, dtype=f64).to(DEV)
-
-
-def fp32(x):                                    # float64 copy of the fp32 value the kernel reads
-    return x.float().double()
-
-
-def fp16(x):
-    return x.to(torch.float16).to(f64)
-
-
-def ulp(x, min_exp, mant):
-    """ulp of a binary float with `mant` explicit mantissa bits and minimum normal exponent min_exp at |x| (float64)."""
-    _, e = torch.frexp(x.abs().clamp_min(2.0 ** min_exp))
-    return torch.ldexp(torch.ones_like(x), e - 1 - mant)
-
-
-def tf32_rna(x):
-    """cvt.rna.tf32.f32 of x (float64 -> fp32 -> tf32, ties away from zero), as float64."""
-    b = x.float().contiguous().view(torch.int32)
-    return ((b + 0x1000) & -0x2000).view(torch.float32).double()
-
-
-def bound(name, got, ref, lim):
-    """|got - ref| <= lim elementwise (lim: float64 tensor of the propagated error); equal infinities pass."""
-    got = got.double()
-    ref = torch.as_tensor(ref, dtype=f64, device=got.device).expand_as(got)
-    lim = torch.as_tensor(lim, dtype=f64, device=got.device).expand_as(got)
-    assert not torch.isnan(got).any(), f"{name}: {int(torch.isnan(got).sum())} elements not written or NaN"
-    same = got == ref
-    err = torch.where(same, torch.zeros_like(got), (got - ref).abs())
-    bad = err > lim
-    if bad.any():
-        i = int(torch.argmax(torch.where(bad, err / lim.clamp_min(1e-300), torch.zeros_like(err)).reshape(-1)))
-        raise AssertionError(f"{name}: {int(bad.sum())}/{bad.numel()} elements out of bound; worst flat index {i}: "
-                             f"got {got.reshape(-1)[i].item():.9g} ref {ref.reshape(-1)[i].item():.9g} "
-                             f"bound {lim.reshape(-1)[i].item():.3g}")
-
-
-def rounded(name, got, ref, err, kind, stats):
-    """A value the kernel rounds to fp16 / tf32 (rna): equal to the rounded reference unless the reference lies within its
-    fp32 error `err` of a rounding boundary (then the kernel's fp32 value may sit on the other side); never more than one
-    ulp (+ err) away."""
-    rnd, u = (fp16, lambda v: ulp(v, -14, 10)) if kind == "fp16" else (tf32_rna, lambda v: ulp(v, -126, 10))
-    got64 = got.double()
-    bound(name, got64, ref, u(torch.maximum(ref.abs(), got64.abs())) + err)
-    straddle = rnd(ref - err) != rnd(ref + err)
-    bad = (got64 != rnd(ref)) & ~straddle
-    assert not bad.any(), (f"{name}: {int(bad.sum())} elements differ from the {kind}-rounded reference away from a "
-                           f"rounding boundary")
-    stats[name] = stats.get(name, 0) + int(straddle.sum())
-
-
 def check(name, got, ref, err, round_out, stats):
     """An output the kernel rounds to tf32 when round_out is set (the float32 twin of the dry run does not round)."""
     if round_out and not CPU:

@@ -20,19 +20,15 @@ not write, or a write past the last row, fails the test.
 PD_TEST_DEV=cpu runs the file with the float32 torch twins of oracle/ref_ops.py in place of the kernels: a dry run of the
 references and tolerances without a GPU."""
 import math
-import os
 from types import SimpleNamespace
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle.ref_ops import RefOps
+from tests.util import CPU, DEV, Gen, bound, f64, fp16, fp32, ops, rounded, ulp  # noqa: F401
 
-DEV = os.environ.get("PD_TEST_DEV", "cuda:0")
-CPU = DEV == "cpu"
 gpu = pytest.mark.gpu if not CPU else (lambda f: f)
-f64 = torch.float64
 EPS = 1e-3                                      # LayerNorm eps of the RSSM (rssm.py: nn.LayerNorm(eps=1e-3))
 # The kernels own one CTA per SM; their limits are functions of that count.  Without a device the dry run uses the count
 # Dreamer._persistent_*_ok assume on the reference path.
@@ -41,45 +37,7 @@ NAN_GUARD = -12345.0                            # sentinel of the guard band aft
 IDX_GUARD = -777
 
 
-@pytest.fixture(scope="module")
-def ops(request):
-    if CPU:
-        return RefOps("cpu")
-    return request.getfixturevalue("native_ops")
-
-
 # ----------------------------------------------------------------------------------------------------- helpers
-class Gen:
-    def __init__(self, seed):
-        self.g = torch.Generator().manual_seed(seed)
-
-    def uniform(self, *shape, bound=1.0):
-        return (torch.rand(*shape, generator=self.g, dtype=f64) * 2 - 1) * bound
-
-    def normal(self, *shape, scale=1.0):
-        return torch.randn(*shape, generator=self.g, dtype=f64) * scale
-
-
-def fp32(x):                                    # float64 copy of the fp32 value the kernel reads
-    return x.float().double()
-
-
-def fp16(x):
-    return x.to(torch.float16).to(f64)
-
-
-def ulp(x, min_exp, mant):
-    """ulp of a binary float with `mant` explicit mantissa bits and minimum normal exponent min_exp at |x| (float64)."""
-    _, e = torch.frexp(x.abs().clamp_min(2.0 ** min_exp))
-    return torch.ldexp(torch.ones_like(x), e - 1 - mant)
-
-
-def tf32_rna(x):
-    """cvt.rna.tf32.f32 of x (float64 -> fp32 -> tf32, ties away from zero), as float64."""
-    b = x.float().contiguous().view(torch.int32)
-    return ((b + 0x1000) & -0x2000).view(torch.float32).double()
-
-
 def guarded(shape, dtype, fill, dev=DEV):
     """A tensor of `shape` pre-filled with `fill`, followed in memory by a sentinel guard band of at least two rows."""
     n = math.prod(shape)
@@ -101,33 +59,6 @@ def check_guards(bufs):
         g = flat[view.numel():]
         sentinel = IDX_GUARD if flat.dtype == torch.int32 else NAN_GUARD
         assert (g == sentinel).all(), f"{name}: written past its last row"
-
-
-def bound(name, got, ref, lim):
-    """|got - ref| <= lim elementwise (lim: float64 tensor of the propagated error)."""
-    got = got.double()
-    assert torch.isfinite(got).all(), f"{name}: {int((~torch.isfinite(got)).sum())} elements not written or not finite"
-    err = (got - ref).abs()
-    bad = err > lim
-    if bad.any():
-        i = int(torch.argmax((err / lim).reshape(-1)))
-        raise AssertionError(f"{name}: {int(bad.sum())}/{bad.numel()} elements out of bound; worst flat index {i}: "
-                             f"got {got.reshape(-1)[i].item():.9g} ref {ref.reshape(-1)[i].item():.9g} "
-                             f"bound {lim.reshape(-1)[i].item():.3g}")
-
-
-def rounded(name, got, ref, err, kind, stats):
-    """A value the kernel rounds to fp16 / tf32 (rna): equal to the rounded reference unless the reference lies within its
-    fp32 error `err` of a rounding boundary (then the kernel's fp32 value may sit on the other side); never more than one
-    ulp (+ err) away."""
-    rnd, u = (fp16, lambda v: ulp(v, -14, 10)) if kind == "fp16" else (tf32_rna, lambda v: ulp(v, -126, 10))
-    got64 = got.double()
-    bound(name, got64, ref, u(torch.maximum(ref.abs(), got64.abs())) + err)
-    straddle = rnd(ref - err) != rnd(ref + err)
-    bad = (got64 != rnd(ref)) & ~straddle
-    assert not bad.any(), (f"{name}: {int(bad.sum())} elements differ from the {kind}-rounded reference away from a "
-                           f"rounding boundary")
-    stats[name] = stats.get(name, 0) + int(straddle.sum())
 
 
 def contraction_tol(scale, trunc=False):
@@ -166,7 +97,7 @@ def ln_stats(x):
 def make_params(D, Hd, G, C, wscale=1.0, seed=0, dev=DEV):
     """fp16-exact weights (uniform +-wscale/sqrt(fan_in), nn.Linear's init times wscale), fp32 biases and LayerNorm affine
     near their init values; all float64 on `dev`."""
-    g = Gen(seed)
+    g = Gen(seed, dev="cpu")
     Z = G * C
 
     def lin(o, i):
@@ -184,7 +115,7 @@ def make_params(D, Hd, G, C, wscale=1.0, seed=0, dev=DEV):
 def make_step_inputs(T, BI, I, D, Hd, G, C, open_loop=False, seed=1, dev=DEV):
     """aa / ea (normal), reset mask (~20% resets, every row reset at step 1), Exp(1) noise, masked h_0 (fp16-exact) and a
     masked one-hot z_0; float64 on `dev`."""
-    g = Gen(seed)
+    g = Gen(seed, dev="cpu")
     B, Z = BI // I, G * C
     mask = (torch.rand(T, BI, generator=g.g) > 0.2).to(f64)
     if T > 1:
@@ -423,7 +354,7 @@ def unroll64(prm, x, T, BI, I, D, Hd, G, C, idx=None):
 
 
 def make_seeds(T, BI, D, Z, seed=3, dev=DEV):
-    g = Gen(seed)
+    g = Gen(seed, dev="cpu")
     return {k: v.to(dev) for k, v in dict(dfeat=fp32(g.normal(T, BI, D + Z, scale=0.1)),
                                           dpost_u=fp32(g.normal(T, BI, Z, scale=0.1)),
                                           w=fp32(0.5 + 0.5 * torch.rand(T, BI, generator=g.g, dtype=f64))).items()}
@@ -587,7 +518,7 @@ def test_persistent_bptt_matches_float64_step_reference(ops, T, BI, D, Hd, G, C,
     kl_weight = 0.8
     prm, x, S = saved_fwd(T, BI, D, Hd, G, C, seed=T + BI + D + G)
     seeds = make_seeds(T, BI, D, Z)
-    gen = Gen(7)
+    gen = Gen(7, dev="cpu")
     gpre = {n: fp32(gen.normal(Hd)).to(DEV) for n in LN_GRADS}         # the gradients ACCUMULATE into these
     o, g = run_bwd(ops, T, BI, D, Hd, G, C, prm, x, S, seeds, kl_weight, bool(round_out), gpre)
     k = {n: v.double() for n, v in o.items()}
