@@ -186,7 +186,8 @@ int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void* stream);
  *   dx1    = LN+ELU backward(in_norm)(dgi . W_ih)                                 rssm.py:138-140
  * Inputs are what pd_rssm_unroll_fwd (or the per-timestep chain) saved; outputs dpost, dy2, dgi, dgh, dx1 [T, BI, .] are the
  * operands of the batched weight-gradient GEMMs, tf32-rounded when round_out != 0.  LayerNorm affine and the two bias
- * gradients fed by LayerNorm inputs are ACCUMULATED (+=) into g_*.  Weights come as TRANSPOSED fp16 copies (pd_transpose_to_half):
+ * gradients fed by LayerNorm inputs are ACCUMULATED (+=) into g_*, in a fixed order (each batch-row owner's partials
+ * go to a row of ws_part2 / ws_part7 after their last use, and the grid adds the rows in order).  Weights come as TRANSPOSED fp16 copies (pd_transpose_to_half):
  * contraction operands carry 10 mantissa bits on both sides (fp16 weights are exact in tf32; gradients are tf32-rounded fp32),
  * like the TF32 GEMMs of the launch chain this replaces.  Limits (P = #CTAs = #SMs; R = min(4, P / G) CTAs per latent
  * group; ks2 / ks6 = 4 when Z resp. 3D is a multiple of 256, else 1): BI <= min(64, P), ceil(BI / R) <= 16, Hd <= 1024,
@@ -205,7 +206,7 @@ typedef struct pd_rssm_bwd_args {
     const float *dfeat, *dpost_u, *w;          /* [T,BI,D+Z] seeds, [T,BI,Z] unweighted KL gradient, [T,BI] row weights */
     float *dpost, *dy2, *dgi, *dgh, *dx1;      /* out [T,BI,Z] [T,BI,Hd] [T,BI,3D] [T,BI,3D] [T,BI,Hd] */
     float *g_ln2_g, *g_ln2_b, *g_b_ph, *g_ln1_g, *g_ln1_b, *g_b_z;   /* += [Hd] each */
-    float *ws_part2, *ws_part6, *ws_part7;     /* workspace [4,BI,Hd] [4,BI,D] [4,BI,Hd] */
+    float *ws_part2, *ws_part6, *ws_part7;     /* workspace [4,BI,Hd] [4,BI,D] [4,BI,Hd]; part2 + part7 also hold the 6 x [BI,Hd] g_* partials */
     unsigned int *ws_barrier;                  /* workspace, 16 words, cleared by the call */
 } pd_rssm_bwd_args;
 int pd_rssm_unroll_bwd(pd_handle* h, const pd_rssm_bwd_args* a, void* stream);
@@ -259,7 +260,8 @@ int pd_bias_act_bwd(pd_handle* h, long M, int N, float* dy, long lddy, const flo
  *   pd_col2im_actbwd:    out = fold(col) .* elu'(dact), dbias[c] += sum over pixels  (Conv2d input gradient; encoders.py:80-90
  *                        backward); out / dact contiguous NHWC [NB, Hout, Wout, Cc], Hout >= 2(Hin-1)+k (rows a stride-2 conv never read get 0)
  * dact is the saved forward output of the layer below (ELU derivative from the output: y > 0 ? 1 : y + 1).
- * Every bias / LayerNorm gradient of this ABI is summed in a fixed order: the same inputs give bit-identical results. */
+ * Every bias / LayerNorm gradient and loss sum of this ABI is added in a fixed order: the same inputs give bit-identical
+ * results. */
 int pd_gemm_actbwd(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_mn, const float* B, long ldb, int b_mn,
                    float* C, long ldc, const float* dact, long lddact, float* dbias, void* stream);
 int pd_conv_gemm_actbwd(pd_handle* h, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo, int o_mn,

@@ -182,12 +182,36 @@ __global__ void colmean_kernel(long M, int N, const float* __restrict__ x, float
 }
 
 // ------------------------------------------------------------------ actor-critic
+// The loss sums in a fixed order: thread q < NQ of every block holds the block's partial q; the partials go to row
+// blockIdx.x of the stream's scratch area and the last block adds them up (a double atomicAdd would add them in arrival
+// order): thread t sums rows t, t + blockDim.x, ... in turn, then the warps and the block reduce in a fixed pattern.
+template <int NQ>
+__device__ __forceinline__ void sums_flush(double v, double* ws, unsigned* ticket, double* sums) {
+    __shared__ double red[NQ][32];
+    if (threadIdx.x < NQ) ws[(long)blockIdx.x * NQ + threadIdx.x] = v;
+    if (!pd_last_block(ticket, gridDim.x)) return;
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) {
+        double s = 0;
+        for (unsigned b = threadIdx.x; b < gridDim.x; b += blockDim.x) s += __ldcg(ws + (long)b * NQ + q);
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) red[q][wp] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < NQ) {
+        double s = 0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[threadIdx.x][w];
+        sums[threadIdx.x] += s;
+    }
+}
+
 constexpr int MAXJ = 128;
 __global__ void gae_critic_kernel(int H, int Md, float gamma, float lambda, const float* __restrict__ vt,
                                   const float* __restrict__ v, const float* __restrict__ rew,
                                   const float* __restrict__ tl, float* __restrict__ term, float* __restrict__ adv,
                                   float* __restrict__ agae, float* __restrict__ target, float* __restrict__ weight,
-                                  float* __restrict__ dv, double* sums) {
+                                  float* __restrict__ dv, double* sums, double* ws, unsigned* ticket) {
     __shared__ double shd[5][8];
     double s_lc = 0, s_v00 = 0, s_v0 = 0, s_r = 0, s_r2 = 0;
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -231,17 +255,17 @@ __global__ void gae_critic_kernel(int H, int Md, float gamma, float lambda, cons
         if (lane == 0) shd[q][wp] = x;
     }
     __syncthreads();
-    if (threadIdx.x < 5) {
-        double x = 0;
+    double x = 0;
+    if (threadIdx.x < 5)
         for (int i = 0; i < (int)(blockDim.x >> 5); ++i) x += shd[threadIdx.x][i];
-        atomicAdd(sums + threadIdx.x, x);
-    }
+    sums_flush<5>(x, ws, ticket, sums);
 }
 
 __global__ void __launch_bounds__(256)
 actor_loss_onehot_kernel(long rows, int A, float eta, const float* __restrict__ logits, long ldl,
                          const float* __restrict__ actions, long lda, const float* __restrict__ agae,
-                         const float* __restrict__ weight, float* __restrict__ dlogits, long lddl, double* sums) {
+                         const float* __restrict__ weight, float* __restrict__ dlogits, long lddl, double* sums,
+                         double* ws, unsigned* ticket) {
     __shared__ double shd[2][8];
     const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
     long row = (long)blockIdx.x * 8 + wp;
@@ -275,17 +299,17 @@ actor_loss_onehot_kernel(long rows, int A, float eta, const float* __restrict__ 
     }
     if (lane == 0) { shd[0][wp] = s_loss; shd[1][wp] = s_ent; }
     __syncthreads();
-    if (threadIdx.x < 2) {
-        double x = 0;
+    double x = 0;
+    if (threadIdx.x < 2)
         for (int i = 0; i < 8; ++i) x += shd[threadIdx.x][i];
-        atomicAdd(sums + threadIdx.x, x);
-    }
+    sums_flush<2>(x, ws, ticket, sums);
 }
 
 __global__ void actor_loss_tanh_normal_kernel(long rows, int A, float eta, const float* __restrict__ out, long ldo,
                                               const float* __restrict__ actions, long lda,
                                               const float* __restrict__ agae, const float* __restrict__ weight,
-                                              float* __restrict__ dout, long lddo, double* sums) {
+                                              float* __restrict__ dout, long lddo, double* sums, double* ws,
+                                              unsigned* ticket) {
     __shared__ double shd[2][8];
     const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
     double s_loss = 0, s_ent = 0;
@@ -321,11 +345,10 @@ __global__ void actor_loss_tanh_normal_kernel(long rows, int A, float eta, const
     }
     if (lane == 0) { shd[0][wp] = s_loss; shd[1][wp] = s_ent; }
     __syncthreads();
-    if (threadIdx.x < 2) {
-        double x = 0;
+    double x = 0;
+    if (threadIdx.x < 2)
         for (int i = 0; i < (int)(blockDim.x >> 5); ++i) x += shd[threadIdx.x][i];
-        atomicAdd(sums + threadIdx.x, x);
-    }
+    sums_flush<2>(x, ws, ticket, sums);
 }
 
 __global__ void tanh_normal_sample_kernel(long rows, int A, const float* __restrict__ out, long ldo,
@@ -493,7 +516,13 @@ int pd_gae_critic(pd_handle* h, int H, int Md, float gamma, float lambda, const 
                   const float* rew, const float* term_logit, float* term, float* adv, float* agae, float* target,
                   float* weight, float* dv, double* sums, void* stream) {
     PD_REQUIRE(h, H >= 1 && H + 1 <= MAXJ, "pd_gae_critic: H=%d unsupported (<%d)", H, MAXJ);
-    gae_critic_kernel<<<pd_cdiv(Md, 128), 128, 0, S(stream)>>>(H, Md, gamma, lambda, vt, v, rew, term_logit, term, adv, agae, target, weight, dv, sums);
+    const int grid = pd_cdiv(Md, 128);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), 2L * grid * 5, 1, &ws, &tk);          // grid x 5 doubles
+    if (rc) return rc;
+    gae_critic_kernel<<<grid, 128, 0, S(stream)>>>(H, Md, gamma, lambda, vt, v, rew, term_logit, term, adv, agae, target, weight, dv, sums,
+                                                   (double*)ws, tk);
     PD_CHECK_LAUNCH(h, "gae_critic");
     return PD_OK;
 }
@@ -501,14 +530,26 @@ int pd_actor_loss_onehot(pd_handle* h, long rows, int A, float eta, const float*
                          long lda, const float* agae, const float* weight, float* dlogits, long lddl, double* sums,
                          void* stream) {
     PD_REQUIRE(h, A >= 1 && A <= 32, "pd_actor_loss_onehot: A=%d unsupported (<=32)", A);
-    actor_loss_onehot_kernel<<<pd_cdiv(rows, 8), 256, 0, S(stream)>>>(rows, A, eta, logits, ldl, actions, lda, agae, weight, dlogits, lddl, sums);
+    const int grid = pd_cdiv(rows, 8);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), 2L * grid * 2, 1, &ws, &tk);          // grid x 2 doubles
+    if (rc) return rc;
+    actor_loss_onehot_kernel<<<grid, 256, 0, S(stream)>>>(rows, A, eta, logits, ldl, actions, lda, agae, weight, dlogits, lddl, sums,
+                                                          (double*)ws, tk);
     PD_CHECK_LAUNCH(h, "actor_loss_onehot");
     return PD_OK;
 }
 int pd_actor_loss_tanh_normal(pd_handle* h, long rows, int A, float eta, const float* out, long ldo,
                               const float* actions, long lda, const float* agae, const float* weight, float* dout,
                               long lddo, double* sums, void* stream) {
-    actor_loss_tanh_normal_kernel<<<pd_cdiv(rows, 256), 256, 0, S(stream)>>>(rows, A, eta, out, ldo, actions, lda, agae, weight, dout, lddo, sums);
+    const int grid = pd_cdiv(rows, 256);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), 2L * grid * 2, 1, &ws, &tk);          // grid x 2 doubles
+    if (rc) return rc;
+    actor_loss_tanh_normal_kernel<<<grid, 256, 0, S(stream)>>>(rows, A, eta, out, ldo, actions, lda, agae, weight, dout, lddo, sums,
+                                                               (double*)ws, tk);
     PD_CHECK_LAUNCH(h, "actor_loss_tanh_normal");
     return PD_OK;
 }

@@ -343,16 +343,29 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
         }
     }
 
-    // ---- flush the LayerNorm / bias gradient accumulators (batch-row owners)
+    // ---- the LayerNorm / bias gradients, added in a fixed order: each batch-row owner writes its six [Hd] accumulators to
+    // row c of a workspace, and after a grid barrier the grid adds rows c = 0..BI-1 in order into g_*.  The rows live in
+    // ws_part2 (quantities 0-3) and ws_part7 (4-5): both are dead once the last P8 has read ws_part7 before barrier (6).
+    auto part = [&](int q, int b) {
+        return q < 4 ? a.ws_part2 + ((long)q * BI + b) * Hd : a.ws_part7 + ((long)(q - 4) * BI + b) * Hd;
+    };
     if (c < BI) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int f = tid + NCT * i;
             if (f < Hd) {
-                atomicAdd(a.g_ln2_g + f, ag2[i]); atomicAdd(a.g_ln2_b + f, ab2[i]); atomicAdd(a.g_b_ph + f, ax2[i]);
-                atomicAdd(a.g_ln1_g + f, ag1[i]); atomicAdd(a.g_ln1_b + f, ab1[i]); atomicAdd(a.g_b_z + f, ax1[i]);
+                part(0, c)[f] = ag2[i]; part(1, c)[f] = ab2[i]; part(2, c)[f] = ax2[i];
+                part(3, c)[f] = ag1[i]; part(4, c)[f] = ab1[i]; part(5, c)[f] = ax1[i];
             }
         }
+    }
+    grid_barrier(a.ws_barrier, epoch);                                          // (7) every owner's partials written
+    float* const gout[6] = {a.g_ln2_g, a.g_ln2_b, a.g_b_ph, a.g_ln1_g, a.g_ln1_b, a.g_b_z};
+    for (int e = c * NCT + tid; e < 6 * Hd; e += P * NCT) {
+        const int q = e / Hd, f = e - q * Hd;
+        float s = 0.f;
+        for (int b = 0; b < BI; ++b) s += __ldcg(part(q, b) + f);
+        gout[q][f] += s;
     }
 }
 

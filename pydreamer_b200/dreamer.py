@@ -907,7 +907,10 @@ class Dreamer(nn.Module):
             for d_, s_ in zip(st["state"], in_state):
                 d_.copy_(s_, non_blocking=True)
         st["graph"].replay()
-        return st["out"]
+        wm_out, ac_out = st["out"]
+        # the captured out_state lives in the graph's memory pool and every replay rewrites it; the caller keeps it as a data
+        # worker's carried state (train.py:177-178, no copy), so it gets its own, as the eager path's clones are
+        return dict(wm_out, out_state=tuple(s_.clone() for s_ in wm_out["out_state"])), ac_out
 
     # ------------------------------------------------------------------ world model forward
     def _rssm_head(self, prior):

@@ -66,6 +66,15 @@ def test_product_arm_tcgen05_teacher_forced_against_oracle(case, persistent):
                                                                                       persistent=persistent)
     assert model._persistent_rssm_ok(conf.batch_size * conf.iwae_samples) == persistent
     assert model._persistent_bptt_ok(conf.batch_size * conf.iwae_samples) == persistent
+    check_teacher_forced_against_oracle(case, conf, obs, state, noise, model, losses, metrics, tensors)
+
+
+def check_teacher_forced_against_oracle(case, conf, obs, state, noise, model, losses, metrics, tensors, target_synced=True,
+                                        tol=1.0):
+    """The step's losses, metrics, every parameter gradient, the reconstructed image and the posterior logits (read from
+    `model` after the four backward calls) against the oracle on the same weights, inputs and noise, teacher-forced on the
+    posterior / prior indices and the actions the GPU sampled.  target_synced: the step copied the critic to its target
+    first (a2c.py:76-79).  tol scales every tolerance (1: those of the TF32 product arm)."""
     T, B, I, H = conf.batch_length, conf.batch_size, conf.iwae_samples, conf.imag_horizon
     N, G, C, D = T * B * I, conf.stoch_dim, conf.stoch_discrete, conf.deter_dim
     post_idx = model._buf("rssm.idx", T, B * I, G, dtype=torch.int32).long().cpu()
@@ -79,14 +88,14 @@ def test_product_arm_tcgen05_teacher_forced_against_oracle(case, persistent):
     flips = int((free["inter"]["post_idx"] != post_idx).sum())
     print(f"[{case}] free-running posterior index flips under TF32: {flips} / {post_idx.numel()}")
     res = O.training_step(sd, conf, cpu(obs), tuple(s.cpu() for s in state), cpu(noise),
-                          force=dict(post_idx=post_idx, actor=actions, prior_idx=prior_idx))
+                          force=dict(post_idx=post_idx, actor=actions, prior_idx=prior_idx), target_synced=target_synced)
     for l in res["losses"]:
         l.backward()
     for i, (got, want) in enumerate(zip(losses, res["losses"])):
         g, w = float(got.detach().reshape(-1)[0]), float(want.detach().reshape(-1)[0])
-        assert abs(g - w) <= 1e-3 * max(1.0, abs(w)), (i, g, w)
+        assert abs(g - w) <= tol * 1e-3 * max(1.0, abs(w)), (i, g, w)
     for k, want in res["metrics"].items():
-        assert abs(float(metrics[k]) - float(want)) <= 2e-3 * max(1.0, abs(float(want))), k
+        assert abs(float(metrics[k]) - float(want)) <= tol * 2e-3 * max(1.0, abs(float(want))), k
     named = dict(model.named_parameters())
     worst = ("", 0.0)
     for k, v in sd.items():
@@ -96,13 +105,13 @@ def test_product_arm_tcgen05_teacher_forced_against_oracle(case, persistent):
         err = abs(g - w) / max(w, 1e-6)
         worst = max(worst, (k, err), key=lambda t: t[1])
         dot = float((named[k].grad.double().cpu() * v.grad.double()).sum()) / max(w * max(g, 1e-12), 1e-12)
-        assert err <= 3e-3 + 1e-7 / max(w, 1e-12), (k, g, w)
+        assert err <= tol * (3e-3 + 1e-7 / max(w, 1e-12)), (k, g, w)
         if w > 1e-6:
             assert dot > 0.999, (k, dot)       # direction of every gradient tensor
     print(f"[{case}] worst grad-norm rel err {worst[1]:.2e} ({worst[0]})")
     rel = lambda a, b: ((a.double().cpu() - b.double()).abs().max() / (b.double().abs().max() + 1e-12)).item()
-    assert rel(tensors["image_rec"], res["tensors"]["image_rec"]) < 2e-3
-    assert rel(model._buf("rssm.post", T, B * I, G * C), res["inter"]["posts"]) < 2e-3
+    assert rel(tensors["image_rec"], res["tensors"]["image_rec"]) < tol * 2e-3
+    assert rel(model._buf("rssm.post", T, B * I, G * C), res["inter"]["posts"]) < tol * 2e-3
 
 
 def test_optimizer_step_and_second_step_on_gpu():

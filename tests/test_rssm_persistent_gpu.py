@@ -539,6 +539,22 @@ def test_persistent_bptt_matches_float64_step_reference(ops, T, BI, D, Hd, G, C,
     print(f"tf32 values within error of a rounding boundary {sum(stats.values())}")
 
 
+@gpu
+@pytest.mark.parametrize("T,BI,D,Hd,G,C", [c for c in BWD_CASES if c.id in ("atari", "BI64_G32_RB16", "T1")])
+def test_persistent_bptt_is_identical_run_to_run(ops, T, BI, D, Hd, G, C):
+    """Two launches on identical inputs and identically pre-filled g_* give bit-identical outputs, the six accumulated
+    LayerNorm / bias gradients included: the batch-row owners' partials are added in row order, not in arrival order."""
+    prm, x, S = saved_fwd(T, BI, D, Hd, G, C, seed=T + BI + D + G)
+    seeds = make_seeds(T, BI, D, G * C)
+    gpre = {n: fp32(Gen(7, dev="cpu").normal(Hd)).to(DEV) for n in LN_GRADS}
+    (o1, g1), (o2, g2) = (run_bwd(ops, T, BI, D, Hd, G, C, prm, x, S, seeds, 0.8, True, gpre) for _ in range(2))
+    for n in o1:
+        assert torch.equal(o1[n].view(torch.int32), o2[n].view(torch.int32)), n
+    for n in LN_GRADS:
+        diff = int((g1[n].view(torch.int32) != g2[n].view(torch.int32)).sum())
+        assert diff == 0, f"g_{n}: {diff}/{Hd} elements differ between two identical launches"
+
+
 def test_bptt_reference_matches_autograd():
     """The float64 step-by-step BPTT formulas against torch.autograd over the whole unrolled float64 forward, with the
     straight-through sample on the reference's own indices (tiny golden shape, every row reset at step 1).  Runs on the
