@@ -297,13 +297,23 @@ int pd_reset_mask(pd_handle* h, int T, int B, int I, const uint8_t* reset, float
 int pd_scalar_head_loss(pd_handle* h, long M, int kind, const float* y, const float* target, int tgt_div,
                         float* loss, float* dy, float* rec, void* stream);
 
+/* Vector-observation head (decoders.py:290-319 DenseNormalDecoder with out_dim = K, std 1/sqrt(2 pi)):
+ *   loss[m] = 0.5 * sum_k (t[k] - y[m,k])^2,   dy[m,k] = y[m,k] - t[k],   target row t = target[m / tgt_div].
+ * One warp per row; each row's sum is added in a fixed order (bit-identical run to run).  y, target, dy are row-strided
+ * (ld in elements).  1 <= K <= PD_VEC_HEAD_MAX_K, ld* >= K, tgt_div >= 1, otherwise PD_ERR_ARG before any launch. */
+#define PD_VEC_HEAD_MAX_K 4096
+int pd_vec_head_loss(pd_handle* h, long M, int K, const float* y, long ldy, const float* target, long ldt, int tgt_div,
+                     float* loss, float* dy, long lddy, void* stream);
+
 /* World-model loss assembly (dreamer.py:362-379, decoders.py:50-108): per (t,b) over I samples.
  * in: per-row losses [TB*I]; out: w[TB*I] = softmax_i(-L)/(TB) (grad of loss_model wrt L_tbi),
- * tb[TB,8] = {loss_model, loss_image, loss_reward, loss_terminal, loss_kl(exact), ent_prior, ent_post, 0}. */
+ * tb[TB,8] = {loss_model, loss_image, loss_reward, loss_terminal, loss_kl(exact), ent_prior, ent_post, loss_vecobs}.
+ * l_img may be NULL (a model without an image decoder: read as 0); l_vec may be NULL (no vector observation: column 7
+ * stays 0), else it enters L with weight w_vec. */
 int pd_wm_loss(pd_handle* h, int TB, int I, float kl_weight, float w_img, float w_rew, float w_term,
                const float* l_img, const float* l_rew, const float* l_term, const float* l_kl,
                const float* kl_exact, const float* ent_prior, const float* ent_post,
-               float* w, float* tb, void* stream);
+               const float* l_vec, float w_vec, float* w, float* tb, void* stream);
 /* out[c] = mean over rows of x[M,N]  (N <= 32) */
 int pd_colmean(pd_handle* h, long M, int N, const float* x, float* out, void* stream);
 

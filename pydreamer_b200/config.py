@@ -37,6 +37,11 @@ SECTIONS = {
     "atari": dict(action_dim=18, clip_rewards="tanh", deter_dim=1024, kl_weight=0.1, gamma=0.99, entropy=0.001),
     # config/defaults.yaml:203-213
     "dmc": dict(action_dim=12, entropy=1.0e-4, actor_grad="dynamics", actor_dist="tanh_normal", clip_rewards="tanh"),
+    # config/defaults.yaml:236-242 (CartPole: a 4-float state vector, no image)
+    "vectorenv": dict(env_id="CartPole-v0", action_dim=2, vecobs_size=4, image_key=None, image_encoder=None,
+                      image_decoder=None),
+    # config/defaults.yaml:244-248 (64x64x3 image + a 27-float vector)
+    "minecraft": dict(env_id="Embodied-minecraft_diamond", action_dim=29, vecobs_size=27, clip_rewards="log1p"),
 }
 
 # BASELINE.json configs (SURVEY.md §0.4: the shipped YAML differs from BASELINE's wording, so the
@@ -52,6 +57,16 @@ PRESETS = {
                               batch_size=3, batch_length=4, imag_horizon=3)),
     "tiny_dmc": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4, action_dim=3,
                                 batch_size=3, batch_length=4, imag_horizon=3, actor_grad="reinforce")),
+    # vector observations as shipped: `vectorenv` has no image encoder / decoder, `minecraft` has both plus the vector
+    "vectorenv": (("vectorenv",), dict()),
+    "minecraft": (("minecraft",), dict()),
+    "tiny_vecobs": (("minecraft",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                         action_dim=5, vecobs_size=27, batch_size=3, batch_length=4, imag_horizon=3)),
+    "tiny_vecobs_iwae3": (("minecraft",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                               action_dim=5, vecobs_size=27, batch_size=3, batch_length=4, imag_horizon=3,
+                                               iwae_samples=3)),
+    "tiny_vector": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
+                                         batch_size=3, batch_length=4, imag_horizon=3)),
 }
 
 

@@ -118,6 +118,27 @@ __global__ void scalar_head_loss_kernel(long M, int kind, const float* __restric
     }
 }
 
+// One warp per row: lane l sums the columns l, l + 32, ... in turn, then the lanes are added by a fixed xor tree, so the
+// loss of a row does not depend on scheduling.
+__global__ void vec_head_loss_kernel(long M, int K, const float* __restrict__ y, long ldy, const float* __restrict__ target,
+                                     long ldt, int div, float* __restrict__ loss, float* __restrict__ dy, long lddy) {
+    const int lane = threadIdx.x & 31;
+    const long warps = (long)gridDim.x * (blockDim.x >> 5);
+    for (long m = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); m < M; m += warps) {
+        const float* yr = y + m * ldy;
+        const float* tr = target + (m / div) * ldt;
+        float s = 0.f;
+        for (int k = lane; k < K; k += 32) {
+            const float d = yr[k] - tr[k];
+            dy[m * lddy + k] = d;
+            s += d * d;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) loss[m] = 0.5f * s;
+    }
+}
+
 __device__ __forceinline__ float neg_logavgexp_neg(const float* v, int I, int stride) {
     // -logavgexp(-v) over I entries (functions.py:97-102); exact passthrough for I == 1
     if (I == 1) return v[0];
@@ -132,12 +153,15 @@ __global__ void wm_loss_kernel(int TB, int I, float kl_weight, float w_img, floa
                                const float* __restrict__ l_img, const float* __restrict__ l_rew,
                                const float* __restrict__ l_term, const float* __restrict__ l_kl,
                                const float* __restrict__ kl_exact, const float* __restrict__ ent_prior,
-                               const float* __restrict__ ent_post, float* __restrict__ w, float* __restrict__ tb) {
+                               const float* __restrict__ ent_post, const float* __restrict__ l_vec, float w_vec,
+                               float* __restrict__ w, float* __restrict__ tb) {
     GRID_STRIDE(r, TB) {
         const long b = r * I;
         float mx = -INFINITY;
         for (int i = 0; i < I; ++i) {
-            float L = kl_weight * l_kl[b + i] + w_img * l_img[b + i] + w_rew * l_rew[b + i] + w_term * l_term[b + i];
+            const float li = l_img ? l_img[b + i] : 0.f;
+            float L = kl_weight * l_kl[b + i] + w_img * li + w_rew * l_rew[b + i] + w_term * l_term[b + i];
+            if (l_vec) L += w_vec * l_vec[b + i];
             w[b + i] = L;
             mx = fmaxf(mx, -L);
         }
@@ -156,13 +180,13 @@ __global__ void wm_loss_kernel(int TB, int I, float kl_weight, float w_img, floa
         for (int i = 0; i < I; ++i) { ep += ent_prior[b + i]; eq += ent_post[b + i]; }
         float* o = tb + r * 8;
         o[0] = loss;
-        o[1] = neg_logavgexp_neg(l_img + b, I, 1);
+        o[1] = l_img ? neg_logavgexp_neg(l_img + b, I, 1) : 0.f;
         o[2] = neg_logavgexp_neg(l_rew + b, I, 1);
         o[3] = neg_logavgexp_neg(l_term + b, I, 1);
         o[4] = neg_logavgexp_neg(kl_exact + b, I, 1);
         o[5] = ep / (float)I;
         o[6] = eq / (float)I;
-        o[7] = 0.f;
+        o[7] = l_vec ? neg_logavgexp_neg(l_vec + b, I, 1) : 0.f;
     }
 }
 
@@ -499,10 +523,21 @@ int pd_scalar_head_loss(pd_handle* h, long M, int kind, const float* y, const fl
     PD_CHECK_LAUNCH(h, "scalar_head_loss");
     return PD_OK;
 }
+int pd_vec_head_loss(pd_handle* h, long M, int K, const float* y, long ldy, const float* target, long ldt, int tgt_div,
+                     float* loss, float* dy, long lddy, void* stream) {
+    PD_REQUIRE(h, M >= 0 && K >= 1 && K <= PD_VEC_HEAD_MAX_K && ldy >= K && ldt >= K && lddy >= K && tgt_div >= 1,
+               "pd_vec_head_loss: K=%d (1..%d), ldy=%ld ldt=%ld lddy=%ld (>= K), tgt_div=%d (>= 1) unsupported", K,
+               PD_VEC_HEAD_MAX_K, ldy, ldt, lddy, tgt_div);
+    if (M == 0) return PD_OK;
+    vec_head_loss_kernel<<<grid_for(M, 8, h->num_sms), 256, 0, S(stream)>>>(M, K, y, ldy, target, ldt, tgt_div, loss, dy, lddy);
+    PD_CHECK_LAUNCH(h, "vec_head_loss");
+    return PD_OK;
+}
 int pd_wm_loss(pd_handle* h, int TB, int I, float kl_weight, float w_img, float w_rew, float w_term, const float* l_img,
                const float* l_rew, const float* l_term, const float* l_kl, const float* kl_exact,
-               const float* ent_prior, const float* ent_post, float* w, float* tb, void* stream) {
-    wm_loss_kernel<<<grid_for(TB, 128, h->num_sms), 128, 0, S(stream)>>>(TB, I, kl_weight, w_img, w_rew, w_term, l_img, l_rew, l_term, l_kl, kl_exact, ent_prior, ent_post, w, tb);
+               const float* ent_prior, const float* ent_post, const float* l_vec, float w_vec, float* w, float* tb,
+               void* stream) {
+    wm_loss_kernel<<<grid_for(TB, 128, h->num_sms), 128, 0, S(stream)>>>(TB, I, kl_weight, w_img, w_rew, w_term, l_img, l_rew, l_term, l_kl, kl_exact, ent_prior, ent_post, l_vec, w_vec, w, tb);
     PD_CHECK_LAUNCH(h, "wm_loss");
     return PD_OK;
 }

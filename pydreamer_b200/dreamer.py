@@ -71,9 +71,9 @@ class _MLP(nn.Module):
 class _DenseHead(nn.Module):
     """decoders.py:257-319 (DenseBernoulliDecoder / DenseNormalDecoder): `.model` is an MLP"""
 
-    def __init__(self, in_dim, hidden_layers, layer_norm, hidden_dim=400):
+    def __init__(self, in_dim, hidden_layers, layer_norm, hidden_dim=400, out_dim=1):
         super().__init__()
-        self.model = _MLP(in_dim, 1, hidden_dim, hidden_layers, layer_norm)
+        self.model = _MLP(in_dim, out_dim, hidden_dim, hidden_layers, layer_norm)
 
 
 class _ConvEncoder(nn.Module):
@@ -87,14 +87,31 @@ class _ConvEncoder(nn.Module):
                                    nn.Flatten())
 
 
+def _image_modules(conf):
+    """True for the conv image encoder + decoder pair, False for a model without image observations."""
+    if conf.image_encoder == "cnn" and conf.image_decoder == "cnn":
+        return True
+    if not conf.image_encoder and not conf.image_decoder:
+        return False
+    raise NotImplementedError(f"accelerated path covers image_encoder / image_decoder both cnn or both empty, not "
+                              f"{conf.image_encoder!r} / {conf.image_decoder!r} (SURVEY.md §2 rows 4-5)")
+
+
 class _MultiEncoder(nn.Module):
+    """encoders.py:10-69: conv embedding of the image and / or an MLP embedding of the vector observation, concatenated
+    image part first."""
+
     def __init__(self, conf):
         super().__init__()
-        if conf.image_encoder != "cnn" or conf.reward_input or conf.vecobs_size:
-            raise NotImplementedError("accelerated path covers image_encoder=cnn without reward_input/vecobs "
-                                      "(SURVEY.md §2 row 4); use the reference for other encoders")
-        self.encoder_image = _ConvEncoder(conf.image_channels, conf.cnn_depth)
-        self.out_dim = self.encoder_image.out_dim
+        if conf.reward_input:
+            raise NotImplementedError("accelerated path covers encoders without reward_input (SURVEY.md §2 row 4)")
+        image = _image_modules(conf)
+        if not image and not conf.vecobs_size:
+            raise AssertionError("Either image_encoder or vecobs_size should be set")      # encoders.py:38
+        self.encoder_image = _ConvEncoder(conf.image_channels, conf.cnn_depth) if image else None
+        self.encoder_vecobs = _MLP(conf.vecobs_size, 256, 400, 2, conf.layer_norm) if conf.vecobs_size else None
+        self.out_dim = ((self.encoder_image.out_dim if image else 0) +
+                        (self.encoder_vecobs.out_dim if conf.vecobs_size else 0))
 
 
 class _ConvDecoder(nn.Module):
@@ -112,14 +129,16 @@ class _ConvDecoder(nn.Module):
 class _MultiDecoder(nn.Module):
     def __init__(self, features_dim, conf):
         super().__init__()
-        if conf.image_decoder != "cnn" or conf.reward_decoder_categorical or conf.vecobs_size:
-            raise NotImplementedError("accelerated path covers image_decoder=cnn + Normal reward head "
-                                      "(SURVEY.md §2 row 5)")
-        if conf.image_size != 64:
+        if conf.reward_decoder_categorical:
+            raise NotImplementedError("accelerated path covers the Normal reward head (SURVEY.md §2 row 5)")
+        image = _image_modules(conf)
+        if image and conf.image_size != 64:
             raise NotImplementedError("conv geometry is the reference's 64x64 one (encoders.py:77-90)")
-        self.image = _ConvDecoder(features_dim, conf.image_channels, conf.cnn_depth)
+        self.image = _ConvDecoder(features_dim, conf.image_channels, conf.cnn_depth) if image else None
         self.reward = _DenseHead(features_dim, conf.reward_decoder_layers, conf.layer_norm)
         self.terminal = _DenseHead(features_dim, conf.terminal_decoder_layers, conf.layer_norm)
+        # decoders.py:66-69: DenseNormalDecoder(out_dim=vecobs_size, hidden_layers=4)
+        self.vecobs = _DenseHead(features_dim, 4, conf.layer_norm, out_dim=conf.vecobs_size) if conf.vecobs_size else None
 
 
 class _GRUStack(nn.Module):
@@ -345,10 +364,15 @@ class Dreamer(nn.Module):
         # static dims
         Aout = conf.action_dim if conf.actor_dist == "onehot" else 2 * conf.action_dim
         cd, IC = conf.cnn_depth, conf.image_channels
+        enc = self.wm.encoder
+        # embedding = cat(image part [Ei], vecobs part [Ev]); each part has its own buffer and meets W_pe's column slice
         self.d = SimpleNamespace(D=conf.deter_dim, G=conf.stoch_dim, C=conf.stoch_discrete,
-                                 Z=conf.stoch_dim * conf.stoch_discrete, Hd=conf.hidden_dim, E=self.wm.encoder.out_dim,
-                                 A=conf.action_dim, F=features_dim, cd=cd, IC=IC, Aout=Aout,
+                                 Z=conf.stoch_dim * conf.stoch_discrete, Hd=conf.hidden_dim, E=enc.out_dim,
+                                 Ei=enc.encoder_image.out_dim if enc.encoder_image is not None else 0,
+                                 Ev=enc.encoder_vecobs.out_dim if enc.encoder_vecobs is not None else 0,
+                                 K=conf.vecobs_size, A=conf.action_dim, F=features_dim, cd=cd, IC=IC, Aout=Aout,
                                  Ap=(Aout + 3) // 4 * 4)   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
+        self._image = enc.encoder_image is not None
         # (input size, output size, in channels, out channels) of the four 4x4 stride-2 convolutions of the encoder
         self._enc_geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
         # (input size, output size, kernel, in channels, out channels) of the four stride-2 deconvolutions of the decoder
@@ -558,25 +582,26 @@ class Dreamer(nn.Module):
         ops.round_copy(self._arena, self._sarena, True)
         if self.fp16_forward:
             ops.to_half(self._arena.view(1, -1), self._harena.view(1, -1))
-        enc = self.wm.encoder.encoder_image.model
-        self._encw = []
-        for li, idx in enumerate((0, 2, 4, 6)):
-            w = enc[idx].weight
-            if li == 0:
-                self._encw.append(self._w(w).view(w.shape[0], -1))          # (c,kh,kw) order == native
-            else:
-                co, ci, kh, kw = w.shape
-                sh = self._buf(f"encw{li}", co, kh, kw, ci)
-                ops.permute4(self._w(w), sh, (0, 2, 3, 1))
-                self._encw.append(sh.view(co, kh * kw * ci))
-        dec = self.wm.decoder.image.model
-        self._decw = []
-        for li, idx in enumerate((2, 4, 6, 8)):
-            w = dec[idx].weight
-            ci, co, kh, kw = w.shape
-            sh = self._buf(f"decw{li}", kh, kw, co, ci)
-            ops.permute4(self._w(w), sh, (2, 3, 1, 0))
-            self._decw.append(sh.view(kh * kw * co, ci))
+        if self._image:
+            enc = self.wm.encoder.encoder_image.model
+            self._encw = []
+            for li, idx in enumerate((0, 2, 4, 6)):
+                w = enc[idx].weight
+                if li == 0:
+                    self._encw.append(self._w(w).view(w.shape[0], -1))          # (c,kh,kw) order == native
+                else:
+                    co, ci, kh, kw = w.shape
+                    sh = self._buf(f"encw{li}", co, kh, kw, ci)
+                    ops.permute4(self._w(w), sh, (0, 2, 3, 1))
+                    self._encw.append(sh.view(co, kh * kw * ci))
+            dec = self.wm.decoder.image.model
+            self._decw = []
+            for li, idx in enumerate((2, 4, 6, 8)):
+                w = dec[idx].weight
+                ci, co, kh, kw = w.shape
+                sh = self._buf(f"decw{li}", kh, kw, co, ci)
+                ops.permute4(self._w(w), sh, (2, 3, 1, 0))
+                self._decw.append(sh.view(kh * kw * co, ci))
         if self.persistent_rssm:      # z_mlp^T [Z, Hd] fp16: a one-hot latent selects rows (persistent unroll, phase A)
             wz = self.wm.core.cell.z_mlp.weight
             self._k1_wzT = self._buf("k1.wzT", wz.shape[1], wz.shape[0], dtype=torch.float16)
@@ -924,29 +949,42 @@ class Dreamer(nn.Module):
         ops, d = self.ops, self.d
         NB, BI = T * B, B * I
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
-        enc = self.wm.encoder.encoder_image.model
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
-        # ---- encoder (encoders.py:72-96): im2col -> tensor-core GEMM (+bias+ELU) x4, NHWC activations
-        img = obs["image"].reshape(NB, d.IC, 64, 64)
-        embed = b("enc.embed", NB, d.E)
         ea = b("rssm.ea", NB, d.Hd)
+        w_pe = self._w(cell.post_mlp_e.weight)         # [Hd, E]: columns [0, Ei) meet the image part, [Ei, E) the vecobs part
+        img = embed = None
         acts, cols = [], []
-        x4 = img.permute(0, 2, 3, 1)
-        for li, (_, hout, ci, co) in enumerate(self._enc_geo):
-            act, col = b(f"enc.a{li}", NB * hout * hout, co), None
-            if li > 0 and self.implicit_conv:
-                ops.conv_gemm(1, x4, 4, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
-            else:
-                col = b(f"enc.col{li}", NB * hout * hout, 16 * ci)
-                ops.im2col(x4, 4, 1 if li == 0 else 0, col, round_out=True)
-                ops.gemm(col, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
-            acts.append(act)
-            cols.append(col)
-            x4 = act.view(NB, hout, hout, co)
-        ops.permute4(x4.view(NB, 4, 8 * d.cd, 1), embed.view(NB, 8 * d.cd, 4, 1), (0, 2, 1, 3),
-                     round_out=True)                                       # (h,w,c) -> reference (c,h,w) flatten
-        ops.gemm(embed, self._w(cell.post_mlp_e.weight), ea)               # hoisted over T
+        if self._image:
+            # ---- encoder (encoders.py:72-96): im2col -> tensor-core GEMM (+bias+ELU) x4, NHWC activations
+            enc = self.wm.encoder.encoder_image.model
+            img = obs["image"].reshape(NB, d.IC, 64, 64)
+            embed = b("enc.embed", NB, d.Ei)
+            x4 = img.permute(0, 2, 3, 1)
+            for li, (_, hout, ci, co) in enumerate(self._enc_geo):
+                act, col = b(f"enc.a{li}", NB * hout * hout, co), None
+                if li > 0 and self.implicit_conv:
+                    ops.conv_gemm(1, x4, 4, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
+                else:
+                    col = b(f"enc.col{li}", NB * hout * hout, 16 * ci)
+                    ops.im2col(x4, 4, 1 if li == 0 else 0, col, round_out=True)
+                    ops.gemm(col, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
+                acts.append(act)
+                cols.append(col)
+                x4 = act.view(NB, hout, hout, co)
+            ops.permute4(x4.view(NB, 4, 8 * d.cd, 1), embed.view(NB, 8 * d.cd, 4, 1), (0, 2, 1, 3),
+                         round_out=True)                                   # (h,w,c) -> reference (c,h,w) flatten
+            ops.gemm(embed, w_pe[:, :d.Ei], ea)                            # hoisted over T
+        vec_in = vembed = venc = None
+        if d.Ev:
+            # ---- vector-observation MLP (encoders.py:33-34, 64-66); its rows of K floats need not be 16-byte multiples,
+            # so its first GEMM (and that layer's weight gradient) take the generic GEMM route
+            vp = self._mlp_params(self.wm.encoder.encoder_vecobs)
+            vec_in = obs["vecobs"].reshape(NB, d.K)
+            vembed = b("enc.vembed", NB, d.Ev)
+            venc = self._mlp_saved(vp, tag + "venc", NB)
+            self._mlp_fwd(vp, vec_in, vembed, venc)
+            ops.gemm(vembed, w_pe[:, d.Ei:], ea, res=ea if self._image else None)     # + the image part's product
 
         # ---- RSSM posterior unroll (rssm.py:21-78, 125-153)
         mask = b("rssm.mask", T, BI)
@@ -962,8 +1000,9 @@ class Dreamer(nn.Module):
         m2, r2 = b("rssm.m2", T, BI), b("rssm.r2", T, BI)
         post = b("rssm.post", T, BI, d.Z)
         idx = b("rssm.idx", T, BI, d.G, dtype=torch.int32)
-        fw = SimpleNamespace(T=T, B=B, I=I, img=img, embed=embed, enc_act=acts, enc_col=cols, mask=mask, hin=hin, zin=zin,
-                             x1=x1, za=za, m1=m1, r1=r1, gates=gates, y2=y2, pin=pin, m2=m2, r2=r2, post=post, idx=idx)
+        fw = SimpleNamespace(T=T, B=B, I=I, img=img, embed=embed, enc_act=acts, enc_col=cols, vec_in=vec_in,
+                             vembed=vembed, venc=venc, mask=mask, hin=hin, zin=zin, x1=x1, za=za, m1=m1, r1=r1,
+                             gates=gates, y2=y2, pin=pin, m2=m2, r2=r2, post=post, idx=idx)
         head = self._rssm_head(prior=open_loop)     # open loop (rssm.py:52-53): the "posterior" is the prior, no embed
         W = self._w
         if self._persistent_rssm_ok(BI):
@@ -1051,17 +1090,22 @@ class Dreamer(nn.Module):
         ops.kl(fw.post.view(N, d.Z), prior, fw.idx.view(N, d.G), 0 if I == 1 else 1, kl_balance_arg(conf.kl_balance), d.G,
                d.C, l_kl, kl_exact, ent_post, ent_prior, fw.dpost_u, fw.dprior)
         fw.w, tb = b("loss.w", N), b("loss.tb", NB, 8)
+        vec = dict(l_vec=dd.l_vec, w_vec=conf.vecobs_weight) if d.K else {}
         ops.wm_loss(NB, I, conf.kl_weight, conf.image_weight, conf.reward_weight, conf.terminal_weight, dd.l_img, dd.l_rew,
-                    dd.l_term, l_kl, kl_exact, ent_prior, ent_post, fw.w, tb)
+                    dd.l_term, l_kl, kl_exact, ent_prior, ent_post, fw.w, tb, **vec)
         means = b("loss.means", 8)
         ops.colmean(tb, means)
         tbv = tb.view(T, B, 8)
-        metrics = dict(loss_image=means[1], loss_reward=means[2], loss_terminal=means[3], loss_model=means[0],
+        metrics = dict(loss_image=means[1]) if self._image else {}
+        metrics.update(loss_reward=means[2], loss_terminal=means[3], loss_model=means[0],
                        loss_kl=means[4], entropy_prior=means[5], entropy_post=means[6])
-        tensors = dict(loss_image=tbv[..., 1], image_rec=self._sel(dd.image, T, B, I), loss_reward=tbv[..., 2],
-                       reward_rec=self._sel(dd.rec_r, T, B, I), loss_terminal=tbv[..., 3],
+        tensors = dict(loss_image=tbv[..., 1], image_rec=self._sel(dd.image, T, B, I)) if self._image else {}
+        tensors.update(loss_reward=tbv[..., 2], reward_rec=self._sel(dd.rec_r, T, B, I), loss_terminal=tbv[..., 3],
                        terminal_rec=self._sel(dd.rec_t, T, B, I), loss_kl=tbv[..., 4], entropy_prior=tbv[..., 5],
                        entropy_post=tbv[..., 6])
+        if d.K:
+            metrics.update(loss_vecobs=means[7])
+            tensors.update(loss_vecobs=tbv[..., 7], vecobs_rec=self._sel(dd.yv, T, B, I))
         if noise_image_pred is not None:
             self._image_pred(obs, fw, prior, noise_image_pred, metrics, tensors)
         return dict(loss_model=means[0], out_state=fw.out_state, metrics=metrics, tensors=tensors), fw
@@ -1084,7 +1128,8 @@ class Dreamer(nn.Module):
         dd = self._decode_all(featP, fw.img, obs, N, NB, I, "p.")
         zeros = b("p.zeros", N, zero=True)
         w, tb = b("p.loss.w", N), b("p.loss.tb", NB, 8)
-        ops.wm_loss(NB, I, 0.0, 1.0, 1.0, 1.0, dd.l_img, dd.l_rew, dd.l_term, zeros, zeros, zeros, zeros, w, tb)
+        vec = dict(l_vec=dd.l_vec, w_vec=1.0) if d.K else {}
+        ops.wm_loss(NB, I, 0.0, 1.0, 1.0, 1.0, dd.l_img, dd.l_rew, dd.l_term, zeros, zeros, zeros, zeros, w, tb, **vec)
         tbv = tb.view(T, B, 8)
         lp_img, lp_rew, lp_term = tbv[..., 1], tbv[..., 2], tbv[..., 3]
         nanmean = lambda x: torch.nansum(x) / (~torch.isnan(x)).sum()                # functions.py:150-151
@@ -1094,11 +1139,17 @@ class Dreamer(nn.Module):
             extra_t[f"logprob_reward{sig}"] = lp_rew * m / m
         m = obs["terminal"] > 0                                                      # decoders.py:103-106
         extra_t["logprob_terminal1"] = lp_term * m / m
-        metrics.update(logprob_image=lp_img.mean(), logprob_reward=lp_rew.mean(), logprob_terminal=lp_term.mean(),
+        if self._image:
+            metrics.update(logprob_image=lp_img.mean())
+            tensors.update(logprob_image=lp_img, image_pred=self._sel(dd.image, T, B, I))
+        metrics.update(logprob_reward=lp_rew.mean(), logprob_terminal=lp_term.mean(),
                        **{k: nanmean(v) for k, v in extra_t.items()})
-        tensors.update(logprob_image=lp_img, logprob_reward=lp_rew, logprob_terminal=lp_term, **extra_t,
-                       image_pred=self._sel(dd.image, T, B, I), reward_pred=self._sel(dd.rec_r, T, B, I),
-                       terminal_pred=self._sel(dd.rec_t, T, B, I))
+        tensors.update(logprob_reward=lp_rew, logprob_terminal=lp_term, **extra_t,
+                       reward_pred=self._sel(dd.rec_r, T, B, I), terminal_pred=self._sel(dd.rec_t, T, B, I))
+        if d.K:
+            lp_vec = tbv[..., 7]
+            metrics.update(logprob_vecobs=lp_vec.mean())
+            tensors.update(logprob_vecobs=lp_vec, vecobs_pred=self._sel(dd.yv, T, B, I))
 
     def _cols_dtype(self, ncols):
         """Column matrices of the transposed convolutions are written once and read once: fp16 halves that traffic.  The GEMM's
@@ -1134,9 +1185,9 @@ class Dreamer(nn.Module):
         """MultiDecoder.training_step forward (decoders.py:50-108) on features (N,F): the image decoder with its loss and the
         reward / terminal MLP heads with theirs.  Buffers are named `tag + ...` (tag "" = the training pass the backward
         reads); returns the image decoder's namespace extended by the heads'."""
-        ops = self.ops
+        ops, d = self.ops, self.d
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
-        dd = self._image_decoder(featN, N, tag, img, I)
+        dd = self._image_decoder(featN, N, tag, img, I) if self._image else SimpleNamespace(l_img=None)
         # reward / terminal heads (decoders.py:257-319)
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
         yr, yt = b("head.yr", N, 1), b("head.yt", N, 1)
@@ -1147,6 +1198,12 @@ class Dreamer(nn.Module):
         dd.l_term, dd.dyt, dd.rec_t = b("loss.term", N), b("head.dyt", N, 1), b("head.rec_t", N)
         ops.scalar_head_loss(0, yr, obs["reward"].reshape(NB), I, dd.l_rew, dd.dyr, dd.rec_r)
         ops.scalar_head_loss(1, yt, obs["terminal"].reshape(NB), I, dd.l_term, dd.dyt, dd.rec_t)
+        if d.K:                              # vector-observation head (decoders.py:66-69, 290-319)
+            vp = self._mlp_params(self.wm.decoder.vecobs.model)
+            dd.yv, dd.vec = b("head.yv", N, d.K), self._mlp_saved(vp, tag + "vec", N)
+            self._mlp_fwd(vp, featN, dd.yv, dd.vec)
+            dd.l_vec, dd.dyv = b("loss.vec", N), b("head.dyv", N, d.K)
+            ops.vec_head_loss(dd.yv, obs["vecobs"].reshape(NB, d.K), I, dd.l_vec, dd.dyv)
         return dd
 
     # ------------------------------------------------------------------ world model backward
@@ -1159,64 +1216,21 @@ class Dreamer(nn.Module):
         b, W, G = self._buf, self._w, self._g
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
-        enc = self.wm.encoder.encoder_image.model
-        dec = self.wm.decoder.image.model
         featN, w, dd = fw.featN, fw.w, fw.dec
         dfeat = b("bwd.dfeat", N, d.F)
+        par_w = self._image and self._ov(4)     # image weight gradients leave the dfeat -> BPTT critical path (joined at the end)
+        if self._image:
+            self._image_decoder_bwd(fw, dfeat, par_w)
 
-        # ---- image decoder backward: seeds = w[n] * image_weight * (dec - target)
-        ops.rowscale(dd.diff.view(N, d.IC * 4096), w, 1, conf.image_weight)
-        ops.rowscale(dd.csum, w, 1, conf.image_weight)
-        ops.colsum(dd.csum, G(dec[8].bias))
-        dgeo = self._dec_geo
-        impl = [self.implicit_conv and li in (1, 2) for li in range(4)]   # deconv 2,3: 32-channel-aligned NHWC gradients
-        copad = [(co + 31) // 32 * 32 if impl[li] else co for li, (_, _, _, _, co) in enumerate(dgeo)]
-        gdec = [b(("bwd.gdecwp" if impl[li] else "bwd.gdecw") + str(li), k * k * copad[li], ci)
-                for li, (_, _, k, ci, _) in enumerate(dgeo)]                 # rows (tap, co padded), as self._decw
-        for g_ in gdec:
-            ops.fill(g_, 0.0)
-        par_w = self._ov(4)                 # weight gradients leave the dfeat -> BPTT critical path (joined at the end)
-        side = (lambda: self._fork(4)) if par_w else contextlib.nullcontext
-        dout4 = dd.diff.permute(0, 2, 3, 1)                    # [n,y,x,c] view of the NCHW diff
-        for li in (3, 2, 1, 0):
-            hi, ho, k, ci, co = dgeo[li]
-            xin = dd.xin[li]
-            dxin = b(f"bwd.dd{li}", N * hi * hi, ci)
-            # (li > 0: the ELU backward and the bias gradient of the deconv below ride in the input-gradient GEMM's epilogue)
-            below_bias = G(dec[2 * li].bias) if li > 0 else None
-            if impl[li]:
-                with side():
-                    ops.conv_gemm(2, dout4, k, xin, gdec[li])                          # weight gradient
-                ops.conv_gemm_actbwd(dout4, k, self._decw[li], dxin, xin, below_bias, o_mn=True)   # input gradient
-            else:
-                if li == 0:
-                    dcols = dout4.reshape(N, k * k * co)       # 5x5 input of a 5x5 kernel: im2col is the identity
-                else:
-                    dcols = b(f"bwd.dcols{li}", N * hi * hi, k * k * co)
-                    ops.im2col(dout4, k, 0, dcols, round_out=True)
-                with side():
-                    ops.gemm(dcols, xin, gdec[li], a_mn=True, b_mn=True, accumulate=True)
-                if li > 0:
-                    ops.gemm_actbwd(dcols, self._decw[li], dxin, xin, below_bias, b_mn=True)
-                else:
-                    ops.gemm(dcols, self._decw[li], dxin, b_mn=True, round_out=True)
-            dout4 = dxin.view(N, hi, hi, ci)
-        dx0 = dxin
-        with side():
-            for li, idx_ in enumerate((2, 4, 6, 8)):          # back to ConvTranspose2d layout (Cin,Cout,kh,kw)
-                wt = dec[idx_].weight
-                ci, co, kh, kw = wt.shape
-                ops.permute4(gdec[li].view(kh, kw, copad[li], ci)[:, :, :co], G(wt), (3, 2, 0, 1))
-            ops.gemm(dx0, featN, G(dec[0].weight), a_mn=True, b_mn=True, accumulate=True)
-            ops.colsum(dx0, G(dec[0].bias))
-        ops.gemm(dx0, W(dec[0].weight), dfeat, b_mn=True)                      # first writer of dfeat
-
-        # ---- reward / terminal heads
+        # ---- reward / terminal heads (without an image decoder the reward head is the first writer of dfeat)
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
         ops.rowscale(dd.dyr, w, 1, conf.reward_weight)
         ops.rowscale(dd.dyt, w, 1, conf.terminal_weight)
-        self._mlp_bwd(rp, featN, dd.dyr, dd.rew, din=dfeat, din_accum=True)
+        self._mlp_bwd(rp, featN, dd.dyr, dd.rew, din=dfeat, din_accum=self._image)
         self._mlp_bwd(tp, featN, dd.dyt, dd.term, din=dfeat, din_accum=True)
+        if d.K:
+            ops.rowscale(dd.dyv, w, 1, conf.vecobs_weight)
+            self._mlp_bwd(self._mlp_params(self.wm.decoder.vecobs.model), featN, dd.dyv, dd.vec, din=dfeat, din_accum=True)
 
         # ---- prior branch (batch_prior): dprior = kl_weight * w[n] * dKL/dprior
         dprior = fw.dprior
@@ -1298,23 +1312,45 @@ class Dreamer(nn.Module):
         else:
             dea, daa = b("bwd.dea", NB, d.Hd), b("bwd.daa", NB, d.Hd)
             ops.group_sum(f2(dy2), I, dea); ops.group_sum(f2(dx1), I, daa)
-        ops.gemm(dea, fw.embed, G(cell.post_mlp_e.weight), a_mn=True, b_mn=True, accumulate=True)
+        g_pe, w_pe = G(cell.post_mlp_e.weight), W(cell.post_mlp_e.weight)     # [Hd, E]: image columns, then vecobs columns
+        if self._image:
+            ops.gemm(dea, fw.embed, g_pe[:, :d.Ei], a_mn=True, b_mn=True, accumulate=True)
+        if d.Ev:
+            ops.gemm(dea, fw.vembed, g_pe[:, d.Ei:], a_mn=True, b_mn=True, accumulate=True)
         ops.gemm(daa, obs["action"].reshape(NB, d.A), G(cell.a_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
 
         # ---- encoder backward
+        dea_c = self._image_encoder_bwd(fw, dy2, w_pe[:, :d.Ei]) if self._image else self._dea_c(fw, dy2)
+        if d.Ev:
+            dembed_v = b("bwd.dembed_v", NB, d.Ev)
+            ops.gemm(dea_c, w_pe[:, d.Ei:], dembed_v, b_mn=True)
+            self._mlp_bwd(self._mlp_params(self.wm.encoder.encoder_vecobs), fw.vec_in, dembed_v, fw.venc)
+        if par_w:
+            self._join(4)
+
+    def _dea_c(self, fw, dy2):
+        """Gradient of the hoisted embedding product ea [T*B, Hd]: dy2 summed over the importance samples."""
+        if fw.I == 1:
+            return dy2.view(-1, self.d.Hd)
+        dea_c = self._buf("bwd.dea_c", fw.T * fw.B, self.d.Hd)
+        self.ops.group_sum(dy2.view(-1, self.d.Hd), fw.I, dea_c)
+        return dea_c
+
+    def _image_encoder_bwd(self, fw, dy2, w_pe_img):
+        """ConvEncoder backward through W_pe's image columns; returns the gradient of ea (_dea_c) it started from."""
+        ops, d = self.ops, self.d
+        NB = fw.T * fw.B
+        b, G = self._buf, self._g
+        enc = self.wm.encoder.encoder_image.model
         geo = self._enc_geo
         cpad = [(ci + 31) // 32 * 32 if self.implicit_conv else ci for _, _, ci, _ in geo]   # implicit: 32 channels per tap
         encgw = {li: b(("bwd.gencwp" if self.implicit_conv else "bwd.gencw") + str(li), geo[li][3], 16 * cpad[li])
                  for li in (1, 2, 3)}
         for li in (1, 2, 3):
             ops.fill(encgw[li], 0.0)
-        if I == 1:
-            dea_c = dy2.view(N, d.Hd)
-        else:
-            dea_c = b("bwd.dea_c", NB, d.Hd)
-            ops.group_sum(dy2.view(N, d.Hd), I, dea_c)
-        dembed = b("bwd.dembed", NB, d.E)
-        ops.gemm(dea_c, W(cell.post_mlp_e.weight), dembed, b_mn=True)
+        dea_c = self._dea_c(fw, dy2)
+        dembed = b("bwd.dembed", NB, d.Ei)
+        ops.gemm(dea_c, w_pe_img, dembed, b_mn=True)
         da = b("bwd.da3", NB * 4, 8 * d.cd)
         ops.permute4(dembed.view(NB, 8 * d.cd, 4, 1), da.view(NB, 4, 8 * d.cd, 1), (0, 2, 1, 3))
         ops.bias_act_bwd(da, fw.enc_act[3], ACT_ELU, G(enc[6].bias))
@@ -1335,8 +1371,60 @@ class Dreamer(nn.Module):
         for li in (1, 2, 3):
             _, _, ci, co = geo[li]
             ops.permute4(encgw[li].view(co, 4, 4, cpad[li])[..., :ci], G(enc[2 * li].weight), (0, 3, 1, 2))
-        if par_w:
-            self._join(4)
+        return dea_c
+
+    def _image_decoder_bwd(self, fw, dfeat, par_w):
+        """ConvDecoder backward: the image-loss seeds w[n] * image_weight * (dec - target) back to the first write of dfeat;
+        with par_w the weight gradients go to side stream 4 (joined by the caller)."""
+        ops, d, conf = self.ops, self.d, self.conf
+        N = fw.T * fw.B * fw.I
+        b, W, G = self._buf, self._w, self._g
+        dec = self.wm.decoder.image.model
+        featN, w, dd = fw.featN, fw.w, fw.dec
+        ops.rowscale(dd.diff.view(N, d.IC * 4096), w, 1, conf.image_weight)
+        ops.rowscale(dd.csum, w, 1, conf.image_weight)
+        ops.colsum(dd.csum, G(dec[8].bias))
+        dgeo = self._dec_geo
+        impl = [self.implicit_conv and li in (1, 2) for li in range(4)]   # deconv 2,3: 32-channel-aligned NHWC gradients
+        copad = [(co + 31) // 32 * 32 if impl[li] else co for li, (_, _, _, _, co) in enumerate(dgeo)]
+        gdec = [b(("bwd.gdecwp" if impl[li] else "bwd.gdecw") + str(li), k * k * copad[li], ci)
+                for li, (_, _, k, ci, _) in enumerate(dgeo)]                 # rows (tap, co padded), as self._decw
+        for g_ in gdec:
+            ops.fill(g_, 0.0)
+        side = (lambda: self._fork(4)) if par_w else contextlib.nullcontext
+        dout4 = dd.diff.permute(0, 2, 3, 1)                    # [n,y,x,c] view of the NCHW diff
+        for li in (3, 2, 1, 0):
+            hi, ho, k, ci, co = dgeo[li]
+            xin = dd.xin[li]
+            dxin = b(f"bwd.dd{li}", N * hi * hi, ci)
+            # (li > 0: the ELU backward and the bias gradient of the deconv below ride in the input-gradient GEMM's epilogue)
+            below_bias = G(dec[2 * li].bias) if li > 0 else None
+            if impl[li]:
+                with side():
+                    ops.conv_gemm(2, dout4, k, xin, gdec[li])                          # weight gradient
+                ops.conv_gemm_actbwd(dout4, k, self._decw[li], dxin, xin, below_bias, o_mn=True)   # input gradient
+            else:
+                if li == 0:
+                    dcols = dout4.reshape(N, k * k * co)       # 5x5 input of a 5x5 kernel: im2col is the identity
+                else:
+                    dcols = b(f"bwd.dcols{li}", N * hi * hi, k * k * co)
+                    ops.im2col(dout4, k, 0, dcols, round_out=True)
+                with side():
+                    ops.gemm(dcols, xin, gdec[li], a_mn=True, b_mn=True, accumulate=True)
+                if li > 0:
+                    ops.gemm_actbwd(dcols, self._decw[li], dxin, xin, below_bias, b_mn=True)
+                else:
+                    ops.gemm(dcols, self._decw[li], dxin, b_mn=True, round_out=True)
+            dout4 = dxin.view(N, hi, hi, ci)
+        dx0 = dxin
+        with side():
+            for li, idx_ in enumerate((2, 4, 6, 8)):          # back to ConvTranspose2d layout (Cin,Cout,kh,kw)
+                wt = dec[idx_].weight
+                ci, co, kh, kw = wt.shape
+                ops.permute4(gdec[li].view(kh, kw, copad[li], ci)[:, :, :co], G(wt), (3, 2, 0, 1))
+            ops.gemm(dx0, featN, G(dec[0].weight), a_mn=True, b_mn=True, accumulate=True)
+            ops.colsum(dx0, G(dec[0].bias))
+        ops.gemm(dx0, W(dec[0].weight), dfeat, b_mn=True)                      # first writer of dfeat
 
     # ------------------------------------------------------------------ imagination rollout
     def _dream(self, feats, N, H, noise_actor, noise_prior, tag):

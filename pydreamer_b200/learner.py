@@ -59,7 +59,7 @@ class Learner:
         from .preprocess import GpuPreprocessor
 
         pre = GpuPreprocessor(self.conf, self.device)
-        keys = ("image", "action", "reward", "terminal", "reset")
+        keys = ("image", "vecobs", "action", "reward", "terminal", "reset")
         metrics = None
         for _, raw in zip(range(num_steps), batches):
             obs = pre.apply({k: raw[k] for k in keys if k in raw})

@@ -353,11 +353,19 @@ class NativeOps:
         self._ck(self.lib.pd_scalar_head_loss(self.h, y.numel(), int(kind), _ptr(y), _ptr(target), int(tgt_div),
                                               _ptr(loss), _ptr(dy), _ptr(rec), self._s()), "pd_scalar_head_loss")
 
+    def vec_head_loss(self, y, target, tgt_div, loss, dy):
+        """loss[m] = 0.5 sum_k (target[m / tgt_div, k] - y[m, k])^2, dy = y - target (row-strided 2-D views)."""
+        M, K = y.shape
+        assert target.shape[1] == K and dy.shape == (M, K) and loss.numel() == M
+        self._ck(self.lib.pd_vec_head_loss(self.h, M, K, _ptr(y), _ld(y), _ptr(target), _ld(target), int(tgt_div),
+                                           _ptr(loss), _ptr(dy), _ld(dy), self._s()), "pd_vec_head_loss")
+
     def wm_loss(self, TB, I, kl_weight, w_img, w_rew, w_term, l_img, l_rew, l_term, l_kl, kl_exact, ent_prior,
-                ent_post, w, tb):
+                ent_post, w, tb, l_vec=None, w_vec=0.0):
         self._ck(self.lib.pd_wm_loss(self.h, TB, I, float(kl_weight), float(w_img), float(w_rew), float(w_term),
                                      _ptr(l_img), _ptr(l_rew), _ptr(l_term), _ptr(l_kl), _ptr(kl_exact),
-                                     _ptr(ent_prior), _ptr(ent_post), _ptr(w), _ptr(tb), self._s()), "pd_wm_loss")
+                                     _ptr(ent_prior), _ptr(ent_post), _ptr(l_vec), float(w_vec), _ptr(w), _ptr(tb),
+                                     self._s()), "pd_wm_loss")
 
     def colmean(self, x, out):
         M, N = x.shape

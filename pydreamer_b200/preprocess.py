@@ -6,6 +6,8 @@ path reads.  The raw replay batch (uint8 HWC images, integer actions, raw reward
     action   int64 (T,B) | fp (T,B,A) -> fp32 one-hot (T,B,A) | as is             preprocessing.py:135-138
     reward   (T,B)                    -> fp32, tanh-clipped if clip_rewards=tanh  preprocessing.py:148-150, functions.py:153-160
     terminal (T,B) -> fp32 ; reset (T,B) bool stays                               preprocessing.py:148
+    vecobs   (T,B,K)                  -> fp32                                     preprocessing.py:160-163
+A batch without `image` (a model without an image encoder) passes without one.
 """
 import torch
 
@@ -31,13 +33,17 @@ class GpuPreprocessor:
         b = {k: (v if isinstance(v, torch.Tensor) else torch.as_tensor(v)).to(dev, non_blocking=True) for k, v in batch.items()}
         T, B = b["reward"].shape[:2]
         out = {}
-        img = b["image"]
-        if img.dtype == torch.uint8:
+        img = b.get("image")
+        if img is None:
+            pass
+        elif img.dtype == torch.uint8:
             H, W, C = img.shape[-3:]
             out["image"] = torch.empty(T, B, C, H, W, device=dev)
             self.ops.image_u8_to_f32(img.contiguous(), out["image"])
         else:
             out["image"] = img.to(torch.float32).movedim(-1, -3).contiguous()
+        if "vecobs" in b:
+            out["vecobs"] = b["vecobs"].to(torch.float32).contiguous()
         act = b["action"]
         if act.dim() == 2:
             out["action"] = torch.empty(T, B, conf.action_dim, device=dev)

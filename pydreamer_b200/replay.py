@@ -5,6 +5,9 @@
   reward   (T,B)         tanh(N(0,1))               clip_rewards: tanh (defaults.yaml:196)
   terminal (T,B)         Bernoulli(0.01) as 0./1.   preprocessing.py:148
   reset    (T,B) bool    reset[0]=True on the first batch, Bernoulli(1/200) elsewhere (data.py:255,284-304)
+  vecobs   (T,B,K)       N(0,1) fp32 when vecobs_size = K > 0  preprocessing.py:160-163
+`image` is left out for a model without an image encoder.  The vecobs draw comes after every other draw, so batches of
+image-only configurations are the same with or without it.
 """
 import torch
 
@@ -25,6 +28,10 @@ def synthetic_batch(conf, seed=1234, T=None, B=None, first=True, device="cpu", p
     if first:
         reset[0] = True
     obs = dict(image=img, action=action, reward=reward, terminal=terminal, reset=reset)
+    if getattr(conf, "vecobs_size", 0):
+        obs["vecobs"] = torch.randn(T, B, conf.vecobs_size, generator=g)
+    if not conf.image_encoder:
+        del obs["image"]
     if pin and torch.cuda.is_available():
         obs = {k: v.pin_memory() for k, v in obs.items()}
     if str(device) != "cpu":
