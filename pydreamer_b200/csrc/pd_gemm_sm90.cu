@@ -2,13 +2,16 @@
 //
 //   C[M,N] (=|+=) sum_k A(m,k) * B(n,k) (+bias)(+residual) -> act
 //
-// Pipeline (one CTA per SM, 288 threads):
+// Pipeline (one CTA per SM, 416 threads):
 //   warp 8      : TMA producer  — cp.async.bulk.tensor tiles (SWIZZLE_128B) into a 5-stage shared-memory ring guarded by
 //                                 full / empty mbarriers
-//   warps 0..7  : consumers     — each owns a 32 x 64 sub-tile of the 128 x 128 output tile: mma.sync m16n8k8 (tf32) or
-//                                 m16n8k16 (fp16) with fp32 accumulators in registers, then the epilogue straight from the
-//                                 registers: bias / residual / ELU / ELU-backward / tf32 rounding -> two 128B-swizzled
-//                                 32 x 32 smem boxes -> TMA store (or TMA reduce-add for accumulate)
+//   warps 9..12 : transposers   — only with an MN-major operand: rewrite each landed MN-major tile in place into the
+//                                 K-major layout, then arrive on the stage's ready mbarrier
+//   warps 0..7  : consumers     — two warpgroups of wgmma.m64n128k8 (tf32) / m64n128k16 (fp16), a warp owns 16 rows x 128
+//                                 columns of the 128 x 128 output tile, fp32 accumulators in registers, one wgmma group in
+//                                 flight; then the epilogue straight from the registers: bias / residual / ELU /
+//                                 ELU-backward / tf32 rounding -> four 128B-swizzled 32 x 16 smem boxes -> TMA store (or
+//                                 TMA reduce-add for accumulate)
 // Work units are (tile, k-split); the producer runs ahead into the next unit while the consumers drain the last.  A tile
 // split over K (few output tiles, long K: weight gradients, one-timestep layers) writes each split's partial tile to a
 // scratch area; the last split of the tile to finish adds the partials in split order and runs the epilogue, so the
@@ -17,8 +20,9 @@
 // Operand layouts: both operands may be K-major ([rows][K], K contiguous) or MN-major ([K][rows]); the second form lets the
 // backward contractions dX = dY*W and dW = dY^T*X read the forward tensors in place (no transposes in HBM).  Every shared
 // tile is made of 128-byte rows with the 16-byte chunk c of row r stored at c ^ (r & 7) (TMA SWIZZLE_128B):
-//   K-major : row = m (or n), 32 fp32 / 64 fp16 k per row; fragments by ldmatrix (conflict-free)
-//   MN-major: row = k, 32 m per row, groups of 32 m 4096 B apart; fragments by scalar loads
+//   K-major : row = m (or n), 32 fp32 / 64 fp16 k per row; read by wgmma through a shared-memory descriptor
+//   MN-major: row = k, 32 m per row, groups of 32 m 4096 B apart; as it lands from TMA, before the transposers turn each
+//             4 KB group into the K-major rows of its 32 m (wgmma reads tf32 operands only K-major)
 // The implicit-GEMM convolution operands (TMA im2col mode on an NHWC tensor) land in the same two layouts.
 #include "pd_common.cuh"
 #include <cuda_fp16.h>
@@ -35,8 +39,11 @@ constexpr int B_BYTES = BN * BK * 4;            // 16 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int GSTR = 4096;                      // bytes between the 32-wide MN groups of an MN-major tile
 constexpr int CONS_WARPS = 8;
-constexpr int NUM_THREADS = 32 * CONS_WARPS + 32;
-constexpr int EPI_STAGING = CONS_WARPS * 2 * 4096;   // per consumer warp: two 32x32 fp32 swizzled TMA-store boxes
+constexpr int TR_WARPS = BM / 32;              // transposer warps: one per 4 KB MN group of a tile
+constexpr int NUM_THREADS = 32 * (CONS_WARPS + 1 + TR_WARPS);
+constexpr int NJ = BN / 8;                      // n8 blocks of a consumer warp's 16 x 128 slice
+constexpr int EPI_ROWS = 16;                    // rows of the epilogue's TMA store boxes: one consumer warp's slice
+constexpr int EPI_STAGING = CONS_WARPS * 2 * 4096;   // per consumer warp: four 32 x 16 fp32 swizzled TMA-store boxes
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + EPI_STAGING;
 static_assert(SMEM_BYTES <= 227 * 1024, "H100 allows 227 KB of shared memory per block");
 
@@ -112,114 +119,102 @@ __device__ __forceinline__ void tma_load_im2col(const void* tmap, uint64_t* bar,
           "h"((uint16_t)off_w), "h"((uint16_t)off_h)
         : "memory");
 }
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_f16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 // byte offset of 16-byte chunk c of row r in a 128B-swizzled tile
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
-// 32-bit element (mn, k) of an MN-major tile (k-rows of 32 mn, groups of 32 mn GSTR apart)
-__device__ __forceinline__ uint32_t ld_mn(const uint8_t* t, int mn, int k) {
-    return *reinterpret_cast<const uint32_t*>(t + (mn >> 5) * GSTR + swz(k, (mn & 31) >> 2) + (mn & 3) * 4);
-}
 
-// One 128-byte k-block of the warp's 32 x 64 sub-tile (rows wm .. wm+31 of the A tile, rows wn .. wn+63 of the B tile):
-// four k-steps of 32 bytes, i.e. m16n8k8 tf32 or m16n8k16 fp16.  K-major fragments come from ldmatrix: viewed as b16 pairs, an
-// 8 x 16-byte block of a K-major tile hands lane (g, t) its element (row g, 32-bit word t) — exactly the tf32 A / B fragment
-// pattern, and for fp16 the standard one.
-__device__ __forceinline__ void mma_kblock(const uint8_t* sa, const uint8_t* sb, int a_mn, int b_mn, int f16, int wm, int wn,
-                                           float (&acc)[2][8][4]) {
-    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, q = lane >> 3, l8 = lane & 7;
+// In-place transpose of one 4 KB block of an MN-major tile (32 k-rows of 32 mn) into the K-major layout the wgmma
+// descriptors read (32 mn-rows of 32 k).  Both layouts are 128B-swizzled and hold the same 32 x 32 elements in the same
+// 4 KB, so one warp transposes a block on its own.  Lane (q, p) = (lane >> 3, lane & 7) moves the two 4 x 4 sub-blocks
+// (mn chunk p, k chunk a = p ^ d), d = 2q and 2q + 1: four 16-byte loads of k-rows 4a .. 4a+3 at chunk p, a transpose in
+// registers, four 16-byte stores of mn-rows 4p .. 4p+3 at chunk a.  The 8 lanes of a quarter-warp (one phase of a
+// 16-byte access) reach 8 different chunk columns on both sides, so neither side has a bank conflict: load r lands in
+// column p ^ r ^ 4 ((p ^ d) & 1), store i in column p ^ d ^ i ^ 4 (p & 1), each a permutation of p.
+__device__ __forceinline__ void transpose_block(uint32_t base, int lane) {
+    const int q = lane >> 3, p = lane & 7;
+    uint32_t v[2][4][4];
 #pragma unroll
-    for (int s = 0; s < 4; ++s) {
-        uint32_t a[2][4];
+    for (int s = 0; s < 2; ++s) {
+        const int a = p ^ (2 * q + s);
 #pragma unroll
-        for (int mi = 0; mi < 2; ++mi) {
-            if (!a_mn) {
-                const int r = wm + mi * 16 + (q & 1) * 8 + l8;
-                ldsm_x4(smem_u32(sa) + swz(r, 2 * s + (q >> 1)), a[mi]);
-            } else {
-                const int m = wm + mi * 16 + g, k = 8 * s + t;
-                a[mi][0] = ld_mn(sa, m, k); a[mi][1] = ld_mn(sa, m + 8, k);
-                a[mi][2] = ld_mn(sa, m, k + 4); a[mi][3] = ld_mn(sa, m + 8, k + 4);
-            }
-        }
+        for (int r = 0; r < 4; ++r)
+            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                         : "=r"(v[s][r][0]), "=r"(v[s][r][1]), "=r"(v[s][r][2]), "=r"(v[s][r][3])
+                         : "r"(base + swz(4 * a + r, p)) : "memory");
+    }
+    __syncwarp();
 #pragma unroll
-        for (int nj = 0; nj < 8; nj += 2) {
-            uint32_t b[4];                                     // b0, b1 of n8-tile nj, then of nj + 1
-            if (!b_mn) {
-                const int r = wn + (nj + (q >> 1)) * 8 + l8;
-                ldsm_x4(smem_u32(sb) + swz(r, 2 * s + (q & 1)), b);
-            } else {
-                const int n = wn + nj * 8 + g, k = 8 * s + t;
-                b[0] = ld_mn(sb, n, k); b[1] = ld_mn(sb, n, k + 4);
-                b[2] = ld_mn(sb, n + 8, k); b[3] = ld_mn(sb, n + 8, k + 4);
-            }
+    for (int s = 0; s < 2; ++s) {
+        const int a = p ^ (2 * q + s);
 #pragma unroll
-            for (int mi = 0; mi < 2; ++mi) {
-                if (f16) { mma_f16(acc[mi][nj], a[mi], b[0], b[1]); mma_f16(acc[mi][nj + 1], a[mi], b[2], b[3]); }
-                else     { mma_tf32(acc[mi][nj], a[mi], b[0], b[1]); mma_tf32(acc[mi][nj + 1], a[mi], b[2], b[3]); }
-            }
-        }
+        for (int i = 0; i < 4; ++i)
+            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};"
+                         ::"r"(base + swz(4 * p + i, a)), "r"(v[s][0][i]), "r"(v[s][1][i]), "r"(v[s][2][i]), "r"(v[s][3][i])
+                         : "memory");
     }
 }
-
 
 // wgmma shared-memory descriptor of a K-major SWIZZLE_128B tile: start >> 4, LBO (unused when swizzled) = 1, SBO = 1024 B
 // between 8-row groups, layout 1 = 128-byte swizzle.
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
     return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// One 128-byte k-block of the warpgroup's 64 x 128 slice (rows 64 wgi .. of the A tile, all 128 rows of the B tile), both
-// operands K-major: four wgmma.m64n128k8 (tf32) / m64n128k16 (fp16), each 32 bytes further along the swizzled rows.  One asm
-// statement from fence to wait, so the compiler never touches the accumulators while the tensor cores own them.  Thread
-// (warp w of the group, lane) holds per n8 block j the same four elements as an mma.sync m16n8 C fragment of rows 16 w ..
-__device__ __forceinline__ void wg_kblock(const uint8_t* sa, const uint8_t* sb, int f16, int wgi, float (&acc)[1][16][4]) {
+
+// The 64 accumulators of a warpgroup's m64n128 slice as read-write asm operands %0 .. %63.  Every asm statement from the
+// first wgmma of a tile to the last wait names all of them, so the compiler never moves or reads them while the tensor
+// cores own them.
+#define PD_ACC4(j) "+f"(acc[j][0]), "+f"(acc[j][1]), "+f"(acc[j][2]), "+f"(acc[j][3])
+#define PD_ACC64 PD_ACC4(0), PD_ACC4(1), PD_ACC4(2), PD_ACC4(3), PD_ACC4(4), PD_ACC4(5), PD_ACC4(6), PD_ACC4(7), \
+                 PD_ACC4(8), PD_ACC4(9), PD_ACC4(10), PD_ACC4(11), PD_ACC4(12), PD_ACC4(13), PD_ACC4(14), PD_ACC4(15)
+#define PD_D64 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28," \
+               "%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54," \
+               "%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+
+// Issues one 128-byte k-block of the warpgroup's 64 x 128 slice (rows 64 wgi .. of the A tile, all 128 rows of the B
+// tile), both tiles K-major, as one wgmma group: four wgmma.m64n128k8 (tf32) / m64n128k16 (fp16), each 32 bytes further
+// along the swizzled rows.  Thread (warp w of the group, lane) holds per n8 block j the same four elements as an mma.sync
+// m16n8 C fragment of rows 16 w ..
+__device__ __forceinline__ void wg_issue(const uint8_t* sa, const uint8_t* sb, int f16, int wgi, float (&acc)[16][4]) {
     const uint64_t a0 = wg_desc(smem_u32(sa) + wgi * 64 * 128), b0 = wg_desc(smem_u32(sb));
     if (f16) {
         asm volatile(
             "{\n\t"
             "wgmma.fence.sync.aligned;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %68, 1, 1, 1, 0, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %65, %69, 1, 1, 1, 0, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %66, %70, 1, 1, 1, 0, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %67, %71, 1, 1, 1, 0, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " PD_D64 ", %64, %68, 1, 1, 1, 0, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " PD_D64 ", %65, %69, 1, 1, 1, 0, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " PD_D64 ", %66, %70, 1, 1, 1, 0, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " PD_D64 ", %67, %71, 1, 1, 1, 0, 0;\n\t"
             "wgmma.commit_group.sync.aligned;\n\t"
-            "wgmma.wait_group.sync.aligned 0;\n\t"
             "}"
-            : "+f"(acc[0][0][0]), "+f"(acc[0][0][1]), "+f"(acc[0][0][2]), "+f"(acc[0][0][3]), "+f"(acc[0][1][0]), "+f"(acc[0][1][1]), "+f"(acc[0][1][2]), "+f"(acc[0][1][3]), "+f"(acc[0][2][0]), "+f"(acc[0][2][1]), "+f"(acc[0][2][2]), "+f"(acc[0][2][3]), "+f"(acc[0][3][0]), "+f"(acc[0][3][1]), "+f"(acc[0][3][2]), "+f"(acc[0][3][3]), "+f"(acc[0][4][0]), "+f"(acc[0][4][1]), "+f"(acc[0][4][2]), "+f"(acc[0][4][3]), "+f"(acc[0][5][0]), "+f"(acc[0][5][1]), "+f"(acc[0][5][2]), "+f"(acc[0][5][3]), "+f"(acc[0][6][0]), "+f"(acc[0][6][1]), "+f"(acc[0][6][2]), "+f"(acc[0][6][3]), "+f"(acc[0][7][0]), "+f"(acc[0][7][1]), "+f"(acc[0][7][2]), "+f"(acc[0][7][3]), "+f"(acc[0][8][0]), "+f"(acc[0][8][1]), "+f"(acc[0][8][2]), "+f"(acc[0][8][3]), "+f"(acc[0][9][0]), "+f"(acc[0][9][1]), "+f"(acc[0][9][2]), "+f"(acc[0][9][3]), "+f"(acc[0][10][0]), "+f"(acc[0][10][1]), "+f"(acc[0][10][2]), "+f"(acc[0][10][3]), "+f"(acc[0][11][0]), "+f"(acc[0][11][1]), "+f"(acc[0][11][2]), "+f"(acc[0][11][3]), "+f"(acc[0][12][0]), "+f"(acc[0][12][1]), "+f"(acc[0][12][2]), "+f"(acc[0][12][3]), "+f"(acc[0][13][0]), "+f"(acc[0][13][1]), "+f"(acc[0][13][2]), "+f"(acc[0][13][3]), "+f"(acc[0][14][0]), "+f"(acc[0][14][1]), "+f"(acc[0][14][2]), "+f"(acc[0][14][3]), "+f"(acc[0][15][0]), "+f"(acc[0][15][1]), "+f"(acc[0][15][2]), "+f"(acc[0][15][3])
+            : PD_ACC64
             : "l"(a0), "l"(a0 + 2), "l"(a0 + 4), "l"(a0 + 6), "l"(b0), "l"(b0 + 2), "l"(b0 + 4), "l"(b0 + 6)
             : "memory");
     } else {
         asm volatile(
             "{\n\t"
             "wgmma.fence.sync.aligned;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %68, 1, 1, 1;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %65, %69, 1, 1, 1;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %66, %70, 1, 1, 1;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %67, %71, 1, 1, 1;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " PD_D64 ", %64, %68, 1, 1, 1;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " PD_D64 ", %65, %69, 1, 1, 1;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " PD_D64 ", %66, %70, 1, 1, 1;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " PD_D64 ", %67, %71, 1, 1, 1;\n\t"
             "wgmma.commit_group.sync.aligned;\n\t"
-            "wgmma.wait_group.sync.aligned 0;\n\t"
             "}"
-            : "+f"(acc[0][0][0]), "+f"(acc[0][0][1]), "+f"(acc[0][0][2]), "+f"(acc[0][0][3]), "+f"(acc[0][1][0]), "+f"(acc[0][1][1]), "+f"(acc[0][1][2]), "+f"(acc[0][1][3]), "+f"(acc[0][2][0]), "+f"(acc[0][2][1]), "+f"(acc[0][2][2]), "+f"(acc[0][2][3]), "+f"(acc[0][3][0]), "+f"(acc[0][3][1]), "+f"(acc[0][3][2]), "+f"(acc[0][3][3]), "+f"(acc[0][4][0]), "+f"(acc[0][4][1]), "+f"(acc[0][4][2]), "+f"(acc[0][4][3]), "+f"(acc[0][5][0]), "+f"(acc[0][5][1]), "+f"(acc[0][5][2]), "+f"(acc[0][5][3]), "+f"(acc[0][6][0]), "+f"(acc[0][6][1]), "+f"(acc[0][6][2]), "+f"(acc[0][6][3]), "+f"(acc[0][7][0]), "+f"(acc[0][7][1]), "+f"(acc[0][7][2]), "+f"(acc[0][7][3]), "+f"(acc[0][8][0]), "+f"(acc[0][8][1]), "+f"(acc[0][8][2]), "+f"(acc[0][8][3]), "+f"(acc[0][9][0]), "+f"(acc[0][9][1]), "+f"(acc[0][9][2]), "+f"(acc[0][9][3]), "+f"(acc[0][10][0]), "+f"(acc[0][10][1]), "+f"(acc[0][10][2]), "+f"(acc[0][10][3]), "+f"(acc[0][11][0]), "+f"(acc[0][11][1]), "+f"(acc[0][11][2]), "+f"(acc[0][11][3]), "+f"(acc[0][12][0]), "+f"(acc[0][12][1]), "+f"(acc[0][12][2]), "+f"(acc[0][12][3]), "+f"(acc[0][13][0]), "+f"(acc[0][13][1]), "+f"(acc[0][13][2]), "+f"(acc[0][13][3]), "+f"(acc[0][14][0]), "+f"(acc[0][14][1]), "+f"(acc[0][14][2]), "+f"(acc[0][14][3]), "+f"(acc[0][15][0]), "+f"(acc[0][15][1]), "+f"(acc[0][15][2]), "+f"(acc[0][15][3])
+            : PD_ACC64
             : "l"(a0), "l"(a0 + 2), "l"(a0 + 4), "l"(a0 + 6), "l"(b0), "l"(b0 + 2), "l"(b0 + 4), "l"(b0 + 6)
             : "memory");
     }
 }
+// Waits until at most N of the warpgroup's wgmma groups are pending.
+template <int N>
+__device__ __forceinline__ void wg_wait(float (&acc)[16][4]) {
+    asm volatile("wgmma.wait_group.sync.aligned %64;" : PD_ACC64 : "n"(N) : "memory");
+}
+#undef PD_ACC4
+#undef PD_ACC64
+#undef PD_D64
 
-// WG: both operands K-major (plain or im2col rows) — two warpgroups of wgmma, a warp owns 16 rows x 128 columns.
-// Otherwise (an MN-major operand: wgmma reads tf32 only K-major) eight mma.sync warps of 32 rows x 64 columns.
-template <bool WG>
+// 8 consumer warps: two warpgroups of wgmma, a warp owns 16 rows x 128 columns of the output tile.  Warp 8: TMA producer.
+// Warps 9 .. 12: with an MN-major operand, transpose each landed stage to K-major (warp 9 + j takes the 4 KB block j of
+// every MN-major tile) and release it to the consumers through ready[]; otherwise they exit at once.
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA3,
@@ -227,11 +222,13 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES + EPI_STAGING);   // [STAGES]
-    uint64_t* empty = full + STAGES;                                            // [STAGES]
+    uint64_t* full = (uint64_t*)(smem + STAGES * STAGE_BYTES + EPI_STAGING);   // [STAGES] TMA landed
+    uint64_t* empty = full + STAGES;                                            // [STAGES] consumers done
+    uint64_t* ready = empty + STAGES;                                           // [STAGES] transposed to K-major
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const bool tr = g.a_mn || g.b_mn;
 
     if (warp == CONS_WARPS && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tmA) : "memory");
@@ -239,7 +236,9 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         if (g.a3_on) asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tmA3) : "memory");
         if (g.b3_on) asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tmB3) : "memory");
         if (g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)&tmC) : "memory");
-        for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONS_WARPS); }
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full[i], 1); mbar_init(&empty[i], CONS_WARPS); mbar_init(&ready[i], TR_WARPS);
+        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -316,50 +315,70 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         return;
     }
 
-    // ===================== consumers: MMA + epilogue =====================
-    constexpr int MI = WG ? 1 : 2, NJ = WG ? 16 : 8;                // m16 x n8 fragments per warp
-    constexpr int RB = 16 * MI;                                      // rows of the warp's slice = rows of its store boxes
+    if (warp > CONS_WARPS) {
+        // ===================== transposers: MN-major tiles -> K-major, in place =====================
+        if (!tr) return;
+        const int blk = (warp - CONS_WARPS - 1) * 4096;
+        int stage = 0; uint32_t phase = 0;
+        for (int u = blockIdx.x; u < units; u += gridDim.x) {
+            const int split = u % g.splits;
+            const int kb1 = min(g.kb_total, (split + 1) * g.kb_per_split);
+            for (int kb = split * g.kb_per_split; kb < kb1; ++kb) {
+                mbar_wait(&full[stage], phase);
+                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+                if (g.a_mn) transpose_block(sa + blk, lane);
+                if (g.b_mn) transpose_block(sa + A_BYTES + blk, lane);
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stores, before wgmma reads them
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&ready[stage]);
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: wgmma + epilogue =====================
     const int g8 = lane >> 2, t4 = lane & 3;
-    const int wm = WG ? (warp >> 2) * 64 + (warp & 3) * 16 : (warp & 3) * 32;   // this warp's slice of the 128 x 128 tile
-    const int wn = WG ? 0 : (warp >> 2) * 64;
+    const int wm = (warp >> 2) * 64 + (warp & 3) * 16;                // this warp's 16 rows of the 128 x 128 tile
     const PdEpilogue& e = g.epi;
-    uint8_t* stg = smem + STAGES * STAGE_BYTES + warp * 2 * 4096;     // NJ / 4 fp32 boxes {32, RB} (or NJ / 8 fp16 {64, RB})
+    uint8_t* stg = smem + STAGES * STAGE_BYTES + warp * 2 * 4096;     // NJ / 4 fp32 boxes {32, 16} (or NJ / 8 fp16 {64, 16})
     int stage = 0; uint32_t phase = 0;
     for (int u = blockIdx.x; u < units; u += gridDim.x) {
         const int tile = u / g.splits, split = u % g.splits;
         const int m0 = (tile / g.num_n) * BM;
         const int n0 = (tile % g.num_n) * BN;
         const int kb1 = min(g.kb_total, (split + 1) * g.kb_per_split);
-        float acc[MI][NJ][4];
+        float acc[NJ][4];
 #pragma unroll
-        for (int mi = 0; mi < MI; ++mi)
+        for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
-            for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                for (int x = 0; x < 4; ++x) acc[mi][nj][x] = 0.f;
+            for (int x = 0; x < 4; ++x) acc[nj][x] = 0.f;
+        // One wgmma group in flight: k-block kb is issued before kb - 1 is waited for, and kb - 1's stage is freed then.
+        int prev = -1;
         for (int kb = split * g.kb_per_split; kb < kb1; ++kb) {
             mbar_wait(&full[stage], phase);
+            if (tr) mbar_wait(&ready[stage], phase);                 // the MN-major tiles are K-major now
             const uint8_t* sa = smem + stage * STAGE_BYTES;
-            if constexpr (WG) wg_kblock(sa, sa + A_BYTES, g.f16, warp >> 2, acc);
-            else              mma_kblock(sa, sa + A_BYTES, g.a_mn, g.b_mn, g.f16, wm, wn, acc);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[stage]);
+            wg_issue(sa, sa + A_BYTES, g.f16, warp >> 2, acc);
+            wg_wait<1>(acc);
+            if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+            prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        wg_wait<0>(acc);
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
 
-        // Fragment element x of (mi, nj): row wm + mi*16 + g8 + 8*(x>>1), column wn + nj*8 + 2*t4 + (x&1).
+        // Fragment element x of nj: row wm + g8 + 8*(x>>1), column nj*8 + 2*t4 + (x&1).
         if (g.splits > 1) {
             // ---- split-K: partial tile to scratch; the last split of the tile sums all partials in split order
             float* tp = g.part + (long)tile * g.splits * (BM * BN);
 #pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
+            for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
-                for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int off = (wm + mi * 16 + g8 + 8 * h) * BN + wn + nj * 8 + 2 * t4;
-                        *reinterpret_cast<float2*>(tp + (long)split * (BM * BN) + off) = make_float2(acc[mi][nj][2 * h], acc[mi][nj][2 * h + 1]);
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    const int off = (wm + g8 + 8 * h) * BN + nj * 8 + 2 * t4;
+                    *reinterpret_cast<float2*>(tp + (long)split * (BM * BN) + off) = make_float2(acc[nj][2 * h], acc[nj][2 * h + 1]);
+                }
             __threadfence();
             asm volatile("bar.sync 1, %0;" ::"n"(32 * CONS_WARPS) : "memory");      // consumer warps only
             __shared__ unsigned s_last;
@@ -371,100 +390,90 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             if (!s_last) continue;
             __threadfence();
 #pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
+            for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
-                for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int off = (wm + mi * 16 + g8 + 8 * h) * BN + wn + nj * 8 + 2 * t4;
-                        float2 sum = make_float2(0.f, 0.f);
-                        for (int sp = 0; sp < g.splits; ++sp) {
-                            const float2 v = __ldcg(reinterpret_cast<const float2*>(tp + (long)sp * (BM * BN) + off));
-                            sum.x += v.x; sum.y += v.y;
-                        }
-                        acc[mi][nj][2 * h] = sum.x; acc[mi][nj][2 * h + 1] = sum.y;
+                for (int h = 0; h < 2; ++h) {
+                    const int off = (wm + g8 + 8 * h) * BN + nj * 8 + 2 * t4;
+                    float2 sum = make_float2(0.f, 0.f);
+                    for (int sp = 0; sp < g.splits; ++sp) {
+                        const float2 v = __ldcg(reinterpret_cast<const float2*>(tp + (long)sp * (BM * BN) + off));
+                        sum.x += v.x; sum.y += v.y;
                     }
+                    acc[nj][2 * h] = sum.x; acc[nj][2 * h + 1] = sum.y;
+                }
         }
         // ---- epilogue
-        const int rbase = m0 + wm, cbase = n0 + wn;
-        if (rbase >= g.M || cbase >= g.N) continue;                  // warp-uniform: nothing of this sub-tile is real
+        const int rbase = m0 + wm, cbase = n0;
+        if (rbase >= g.M || cbase >= g.N) continue;                  // warp-uniform: nothing of this slice is real
 #pragma unroll
-        for (int mi = 0; mi < MI; ++mi)
+        for (int nj = 0; nj < NJ; ++nj)
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
+                const int row = rbase + g8 + 8 * (x >> 1), col = cbase + nj * 8 + 2 * t4 + (x & 1);
+                float v = acc[nj][x];
+                const bool in = row < g.M && col < g.N;
+                if (!e.accumulate && in) {
+                    if (e.bias) v += __ldg(e.bias + col);
+                    if (e.R) v += __ldg(e.R + (long)(row / e.r_div) * e.ldr + col);
+                }
+                if (g.tma_store || !e.accumulate) {
+                    if (e.act == PD_ACT_ELU) v = pd_elu(v);
+                    if (e.dact && in) v *= pd_elu_grad_from_out(__ldg(e.dact + (long)row * e.lddact + col));
+                    if (e.round_out) v = pd_tf32(v);
+                }
+                acc[nj][x] = v;
+            }
+        if (!g.tma_store) {
+            // generic path (C not TMA-addressable: ldc % 4 != 0, e.g. N = 1 / 18 outputs)
 #pragma unroll
             for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
                 for (int x = 0; x < 4; ++x) {
-                    const int row = rbase + mi * 16 + g8 + 8 * (x >> 1), col = cbase + nj * 8 + 2 * t4 + (x & 1);
-                    float v = acc[mi][nj][x];
-                    const bool in = row < g.M && col < g.N;
-                    if (!e.accumulate && in) {
-                        if (e.bias) v += __ldg(e.bias + col);
-                        if (e.R) v += __ldg(e.R + (long)(row / e.r_div) * e.ldr + col);
+                    const int row = rbase + g8 + 8 * (x >> 1), col = cbase + nj * 8 + 2 * t4 + (x & 1);
+                    if (row < g.M && col < g.N) {
+                        float* cp = e.C + (long)row * e.ldc + col;
+                        if (e.accumulate) atomicAdd(cp, acc[nj][x]);
+                        else *cp = acc[nj][x];
                     }
-                    if (g.tma_store || !e.accumulate) {
-                        if (e.act == PD_ACT_ELU) v = pd_elu(v);
-                        if (e.dact && in) v *= pd_elu_grad_from_out(__ldg(e.dact + (long)row * e.lddact + col));
-                        if (e.round_out) v = pd_tf32(v);
-                    }
-                    acc[mi][nj][x] = v;
                 }
-        if (!g.tma_store) {
-            // generic path (C not TMA-addressable: ldc % 4 != 0, e.g. N = 1 / 18 outputs)
-#pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
-#pragma unroll
-                for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                    for (int x = 0; x < 4; ++x) {
-                        const int row = rbase + mi * 16 + g8 + 8 * (x >> 1), col = cbase + nj * 8 + 2 * t4 + (x & 1);
-                        if (row < g.M && col < g.N) {
-                            float* cp = e.C + (long)row * e.ldc + col;
-                            if (e.accumulate) atomicAdd(cp, acc[mi][nj][x]);
-                            else *cp = acc[mi][nj][x];
-                        }
-                    }
             continue;
         }
         if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // staging boxes free again
         __syncwarp();
         const uint32_t sbase = smem_u32(stg);
         if (e.c_f16) {
-            // NJ / 8 boxes {64 halfs, RB rows}: 128-byte rows, 16-byte chunk = 8 columns
+            // NJ / 8 boxes {64 halfs, 16 rows}: 128-byte rows, 16-byte chunk = 8 columns
 #pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
+            for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
-                for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int r = mi * 16 + g8 + 8 * h;
-                        const __half2 v2 = __floats2half2_rn(acc[mi][nj][2 * h], acc[mi][nj][2 * h + 1]);
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (nj >> 3) * (RB * 128) + swz(r, nj & 7) + t4 * 4),
-                                     "r"(*reinterpret_cast<const uint32_t*>(&v2))
-                                     : "memory");
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    const int r = g8 + 8 * h;
+                    const __half2 v2 = __floats2half2_rn(acc[nj][2 * h], acc[nj][2 * h + 1]);
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(sbase + (nj >> 3) * (EPI_ROWS * 128) + swz(r, nj & 7) + t4 * 4),
+                                 "r"(*reinterpret_cast<const uint32_t*>(&v2))
+                                 : "memory");
+                }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
             if (lane == 0) {
                 for (int b = 0; b < NJ / 8 && cbase + 64 * b < g.N; ++b)
                     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (RB * 128)), "r"(cbase + 64 * b), "r"(rbase) : "memory");
+                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (EPI_ROWS * 128)), "r"(cbase + 64 * b), "r"(rbase) : "memory");
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
             continue;
         }
-        // NJ / 4 boxes {32 fp32, RB rows}: box b holds columns 32b .. 32b+31 of the slice
+        // NJ / 4 boxes {32 fp32, 16 rows}: box b holds columns 32b .. 32b+31 of the slice
 #pragma unroll
-        for (int mi = 0; mi < MI; ++mi)
+        for (int nj = 0; nj < NJ; ++nj)
 #pragma unroll
-            for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = mi * 16 + g8 + 8 * h, lc = (nj & 3) * 8 + 2 * t4;
-                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};"
-                                 ::"r"(sbase + (nj >> 2) * (RB * 128) + swz(r, lc >> 2) + (lc & 3) * 4), "f"(acc[mi][nj][2 * h]),
-                                   "f"(acc[mi][nj][2 * h + 1])
-                                 : "memory");
-                }
+            for (int h = 0; h < 2; ++h) {
+                const int r = g8 + 8 * h, lc = (nj & 3) * 8 + 2 * t4;
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};"
+                             ::"r"(sbase + (nj >> 2) * (EPI_ROWS * 128) + swz(r, lc >> 2) + (lc & 3) * 4), "f"(acc[nj][2 * h]),
+                               "f"(acc[nj][2 * h + 1])
+                             : "memory");
+            }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         const int nbox = min(NJ / 4, (g.N - cbase + 31) / 32);
@@ -472,10 +481,10 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             for (int b = 0; b < nbox; ++b) {
                 if (e.accumulate)
                     asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];"
-                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (RB * 128)), "r"(cbase + 32 * b), "r"(rbase) : "memory");
+                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (EPI_ROWS * 128)), "r"(cbase + 32 * b), "r"(rbase) : "memory");
                 else
                     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (RB * 128)), "r"(cbase + 32 * b), "r"(rbase) : "memory");
+                                 ::"l"((uint64_t)&tmC), "r"(sbase + b * (EPI_ROWS * 128)), "r"(cbase + 32 * b), "r"(rbase) : "memory");
             }
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
@@ -548,15 +557,9 @@ int make_im2col_map(pd_handle* h, CUtensorMap* tm, const float* base, int NB, in
     return PD_OK;
 }
 
-// wgmma reads tf32 operands only K-major: both operands K-major (plain, fp16 or im2col rows) take the wgmma instantiation.
-bool wgmma_ok(const GemmArgs& g) { return !g.a_mn && !g.b_mn && g.a_mode != 2 && g.b_mode != 2; }
-// rows of the epilogue's TMA store boxes: one warp's slice (16 rows under wgmma, 32 under mma.sync)
-uint32_t store_rows(const GemmArgs& g) { return wgmma_ok(g) ? 16 : 32; }
-
 int configure(pd_handle* h) {
     if (h->gemm_smem_configured) return PD_OK;
-    cudaError_t e = cudaFuncSetAttribute(pd_gemm_tf32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(pd_gemm_tf32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(pd_gemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) PD_FAIL(h, PD_ERR_DEVICE, "cudaFuncSetAttribute(smem=%d): %s", SMEM_BYTES, cudaGetErrorString(e));
     h->gemm_smem_configured = 1;
     return PD_OK;
@@ -594,8 +597,7 @@ int launch(pd_handle* h, const CUtensorMap& tmA, const CUtensorMap& tmB, const C
     }
     const int units = tiles * g.splits;
     const int grid = units < h->num_sms ? units : h->num_sms;
-    if (wgmma_ok(g)) pd_gemm_tf32_kernel<true><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmA, tmB, tmC, tmA3, tmB3, g);
-    else             pd_gemm_tf32_kernel<false><<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmA, tmB, tmC, tmA3, tmB3, g);
+    pd_gemm_tf32_kernel<<<grid, NUM_THREADS, SMEM_BYTES, stream>>>(tmA, tmB, tmC, tmA3, tmB3, g);
     PD_CHECK_LAUNCH(h, name);
     return PD_OK;
 }
@@ -647,7 +649,7 @@ int pd_conv_gemm_launch(pd_handle* h, int mode, int NB, int H, int W, int C, int
         rc = make_map3(h, &tmA3, O, (uint64_t)M, (uint64_t)pixels, (uint64_t)ldo, &g.a3_on, &g.a3_part); if (rc) return rc;
         rc = make_im2col_map(h, &tmB, X, NB, H, W, C, k, BK); if (rc) return rc;
     }
-    rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 32, store_rows(g));
+    rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 32, EPI_ROWS);
     if (rc) return rc;
     g.M = M; g.N = N; g.K = 0;
     g.num_m = pd_cdiv(M, BM); g.num_n = pd_cdiv(N, BN);
@@ -689,10 +691,10 @@ int pd_gemm_tc_launch(pd_handle* h, int M, int N, int K, const void* A, long lda
         PD_REQUIRE(h, !epi.accumulate && !epi.R && !epi.round_out, "pd_gemm: an fp16 output takes bias / activation only");
         PD_REQUIRE(h, (epi.ldc % 8) == 0 && ((((uintptr_t)epi.C) & 15) == 0), "pd_gemm: fp16 output needs ldc %% 8 == 0 (16-byte rows)");
         g.tma_store = 1;
-        rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 64, store_rows(g), 2);
+        rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 64, EPI_ROWS, 2);
         if (rc) return rc;
     } else if (g.tma_store) {
-        rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 32, store_rows(g));
+        rc = make_map(h, &tmC, epi.C, (uint64_t)N, (uint64_t)M, (uint64_t)epi.ldc, 32, EPI_ROWS);
         if (rc) return rc;
     } else {
         tmC = tmA;
