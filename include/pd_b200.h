@@ -305,6 +305,19 @@ int pd_scalar_head_loss(pd_handle* h, long M, int kind, const float* y, const fl
 int pd_vec_head_loss(pd_handle* h, long M, int K, const float* y, long ldy, const float* target, long ldt, int tgt_div,
                      float* loss, float* dy, long lddy, void* stream);
 
+/* Categorical reward head on a support s[S] (decoders.py:322-362 DenseCategoricalSupportDecoder, common.py:77-86
+ * CategoricalSupport.mean): for M rows of S logits y (row pitch ldy), p = softmax(y[m]),
+ *   rec[m]  = sum_k p_k s_k                                    (the expected reward; NULL allowed when target is given)
+ * and, with a target (row m reads target[m / tgt_div]):
+ *   k*      = argmin_k (t - s_k)^2 in fp32, the first index on ties (to_categorical, decoders.py:349-352),
+ *   loss[m] = logsumexp(y[m]) - y[m, k*],   dy[m, k] = p_k - [k == k*] (pitch lddy),   idx[m] = k* (int32, optional).
+ * A NULL target is the expectation-only mode (rewards of the imagination rollout): only rec is written.  One warp per
+ * row; every sum of a row is added in a fixed order.  2 <= S <= PD_SUPPORT_MAX, ldy >= S, tgt_div >= 1, with a target
+ * loss, dy and lddy >= S, without one rec; otherwise PD_ERR_ARG before any launch. */
+#define PD_SUPPORT_MAX 1024
+int pd_support_head(pd_handle* h, long M, int S, const float* y, long ldy, const float* support, const float* target,
+                    int tgt_div, float* rec, float* loss, float* dy, long lddy, int* idx, void* stream);
+
 /* World-model loss assembly (dreamer.py:362-379, decoders.py:50-108): per (t,b) over I samples.
  * in: per-row losses [TB*I]; out: w[TB*I] = softmax_i(-L)/(TB) (grad of loss_model wrt L_tbi),
  * tb[TB,8] = {loss_model, loss_image, loss_reward, loss_terminal, loss_kl(exact), ent_prior, ent_post, loss_vecobs}.

@@ -67,6 +67,24 @@ PRESETS = {
                                                iwae_samples=3)),
     "tiny_vector": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
                                          batch_size=3, batch_length=4, imag_horizon=3)),
+    # the categorical reward head (reward_decoder_categorical): Atari's [-1, 0, 1] through tanh clipping, S = 3
+    "atari_catreward": (("atari",), dict(deter_dim=2048, batch_size=50, batch_length=50,
+                                         reward_decoder_categorical=[-1.0, 0.0, 1.0])),
+    "tiny_catreward": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                        action_dim=5, batch_size=3, batch_length=4, imag_horizon=3,
+                                        reward_decoder_categorical=[-1.0, 0.0, 1.0])),
+    "tiny_catreward_iwae3": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                              action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, iwae_samples=3,
+                                              reward_decoder_categorical=[-1.0, 0.0, 1.0])),
+    "tiny_dmc_catreward": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                          action_dim=3, batch_size=3, batch_length=4, imag_horizon=3,
+                                          actor_grad="reinforce", clip_rewards=None, reward_decoder_categorical=[0, 1])),
+    # 33 unsorted support values (a row pitch of 36), every value in [-1, 0.875] listed twice: the target bucket of almost
+    # every reward is a tie that the first index wins
+    "tiny_catreward_wide": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                             action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, clip_rewards=None,
+                                             reward_decoder_categorical=[((5 * i) % 17 - 8) / 8 for i in range(17)] +
+                                             [((3 * i) % 16 - 8) / 8 for i in range(16)])),
 }
 
 

@@ -139,6 +139,58 @@ __global__ void vec_head_loss_kernel(long M, int K, const float* __restrict__ y,
     }
 }
 
+// One warp per row, as vec_head_loss_kernel: lane l takes the columns l, l + 32, ... in turn and the lanes meet in a fixed
+// xor tree (every lane ends with the same sums).  The target bucket compares (t - s_k)^2 rounded as torch computes it
+// (a subtraction and a multiplication, no FMA contraction); a lane keeps its first minimum and the tree prefers the lower
+// index on equal distances, so k* is the first index of the minimum, as torch.argmin returns.
+__global__ void support_head_kernel(long M, int S, const float* __restrict__ y, long ldy, const float* __restrict__ sup,
+                                    const float* __restrict__ target, int div, float* __restrict__ rec,
+                                    float* __restrict__ loss, float* __restrict__ dy, long lddy, int* __restrict__ idx) {
+    const int lane = threadIdx.x & 31;
+    const long warps = (long)gridDim.x * (blockDim.x >> 5);
+    for (long m = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); m < M; m += warps) {
+        const float* yr = y + m * ldy;
+        float mx = -INFINITY;
+        for (int k = lane; k < S; k += 32) mx = fmaxf(mx, yr[k]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        float z = 0.f, zs = 0.f;
+        for (int k = lane; k < S; k += 32) {
+            const float e = expf(yr[k] - mx);
+            z += e;
+            zs += e * sup[k];
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            z += __shfl_xor_sync(0xffffffffu, z, o);
+            zs += __shfl_xor_sync(0xffffffffu, zs, o);
+        }
+        if (rec && lane == 0) rec[m] = zs / z;
+        if (!target) continue;
+        const float t = target[m / div];
+        float bd = 0.f;
+        int bk = -1;
+        for (int k = lane; k < S; k += 32) {
+            const float d = __fsub_rn(t, sup[k]);
+            const float q = __fmul_rn(d, d);
+            if (bk < 0 || q < bd) { bd = q; bk = k; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float od = __shfl_xor_sync(0xffffffffu, bd, o);
+            const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
+            if (ok >= 0 && (bk < 0 || od < bd || (od == bd && ok < bk))) { bd = od; bk = ok; }
+        }
+        bk = __shfl_sync(0xffffffffu, bk, 0);
+        const float inv = 1.f / z;
+        for (int k = lane; k < S; k += 32) dy[m * lddy + k] = expf(yr[k] - mx) * inv - (k == bk ? 1.f : 0.f);
+        if (lane == 0) {
+            loss[m] = (mx + logf(z)) - yr[bk];
+            if (idx) idx[m] = bk;
+        }
+    }
+}
+
 __device__ __forceinline__ float neg_logavgexp_neg(const float* v, int I, int stride) {
     // -logavgexp(-v) over I entries (functions.py:97-102); exact passthrough for I == 1
     if (I == 1) return v[0];
@@ -531,6 +583,19 @@ int pd_vec_head_loss(pd_handle* h, long M, int K, const float* y, long ldy, cons
     if (M == 0) return PD_OK;
     vec_head_loss_kernel<<<grid_for(M, 8, h->num_sms), 256, 0, S(stream)>>>(M, K, y, ldy, target, ldt, tgt_div, loss, dy, lddy);
     PD_CHECK_LAUNCH(h, "vec_head_loss");
+    return PD_OK;
+}
+int pd_support_head(pd_handle* h, long M, int S, const float* y, long ldy, const float* support, const float* target,
+                    int tgt_div, float* rec, float* loss, float* dy, long lddy, int* idx, void* stream) {
+    PD_REQUIRE(h, M >= 0 && S >= 2 && S <= PD_SUPPORT_MAX && ldy >= S && tgt_div >= 1 && y && support,
+               "pd_support_head: S=%d (2..%d), ldy=%ld (>= S), tgt_div=%d (>= 1) unsupported", S, PD_SUPPORT_MAX, ldy,
+               tgt_div);
+    PD_REQUIRE(h, target ? (loss && dy && lddy >= S) : (rec != nullptr),
+               "pd_support_head: a target needs loss and dy (lddy=%ld >= S), no target needs rec", lddy);
+    if (M == 0) return PD_OK;
+    support_head_kernel<<<grid_for(M, 8, h->num_sms), 256, 0, S(stream)>>>(M, S, y, ldy, support, target, tgt_div, rec,
+                                                                           loss, dy, lddy, idx);
+    PD_CHECK_LAUNCH(h, "support_head");
     return PD_OK;
 }
 int pd_wm_loss(pd_handle* h, int TB, int I, float kl_weight, float w_img, float w_rew, float w_term, const float* l_img,

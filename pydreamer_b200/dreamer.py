@@ -20,11 +20,12 @@ import os
 import warnings
 from types import SimpleNamespace
 
+import numpy as np
 import torch
 import torch.nn as nn
 
 from . import ops as _ops
-from .ops import ACT_ELU, ACT_NONE
+from .ops import ACT_ELU, ACT_NONE, SUPPORT_MAX
 
 
 def kl_balance_arg(kl_balance):
@@ -74,6 +75,36 @@ class _DenseHead(nn.Module):
     def __init__(self, in_dim, hidden_layers, layer_norm, hidden_dim=400, out_dim=1):
         super().__init__()
         self.model = _MLP(in_dim, out_dim, hidden_dim, hidden_layers, layer_norm)
+
+
+def _clip_rewards_np(x, type_):
+    """functions.py:153-160"""
+    if not type_:
+        return x
+    with np.errstate(all="ignore"):            # log1p(-1) = -inf: refused by _SupportHead with a clearer message
+        if type_ == "tanh":
+            return np.tanh(x)
+        if type_ == "log1p":
+            return np.log1p(x)
+    raise AssertionError(type_)
+
+
+class _SupportHead(nn.Module):
+    """decoders.py:322-336 (DenseCategoricalSupportDecoder): `.model` is an MLP with one logit per support value;
+    `_support` holds the support as a parameter that is never trained (its .grad stays None)."""
+
+    def __init__(self, in_dim, support, hidden_layers, layer_norm):
+        if not isinstance(support, (list, np.ndarray)):
+            raise AssertionError()                                                     # decoders.py:329
+        if not 2 <= len(support) <= SUPPORT_MAX:
+            raise NotImplementedError(f"reward_decoder_categorical: {len(support)} support values; the categorical reward "
+                                      f"head takes 2 to {SUPPORT_MAX}")
+        super().__init__()
+        self.model = _MLP(in_dim, len(support), 400, hidden_layers, layer_norm)
+        self._support = nn.Parameter(torch.tensor(support).to(torch.float), requires_grad=False)
+        if not torch.isfinite(self._support).all():
+            raise ValueError(f"reward_decoder_categorical: the support after clip_rewards is not finite: "
+                             f"{self._support.tolist()}")
 
 
 class _ConvEncoder(nn.Module):
@@ -129,13 +160,15 @@ class _ConvDecoder(nn.Module):
 class _MultiDecoder(nn.Module):
     def __init__(self, features_dim, conf):
         super().__init__()
-        if conf.reward_decoder_categorical:
-            raise NotImplementedError("accelerated path covers the Normal reward head (SURVEY.md §2 row 5)")
         image = _image_modules(conf)
         if image and conf.image_size != 64:
             raise NotImplementedError("conv geometry is the reference's 64x64 one (encoders.py:77-90)")
         self.image = _ConvDecoder(features_dim, conf.image_channels, conf.cnn_depth) if image else None
-        self.reward = _DenseHead(features_dim, conf.reward_decoder_layers, conf.layer_norm)
+        if conf.reward_decoder_categorical:         # decoders.py:34-40: the support values are clipped like rewards
+            self.reward = _SupportHead(features_dim, _clip_rewards_np(conf.reward_decoder_categorical, conf.clip_rewards),
+                                       conf.reward_decoder_layers, conf.layer_norm)
+        else:
+            self.reward = _DenseHead(features_dim, conf.reward_decoder_layers, conf.layer_norm)
         self.terminal = _DenseHead(features_dim, conf.terminal_decoder_layers, conf.layer_norm)
         # decoders.py:66-69: DenseNormalDecoder(out_dim=vecobs_size, hidden_layers=4)
         self.vecobs = _DenseHead(features_dim, 4, conf.layer_norm, out_dim=conf.vecobs_size) if conf.vecobs_size else None
@@ -289,10 +322,12 @@ class _FusedAdamW:
         o._grads_pending.discard(self.gid)
 
     def _slices(self):
-        """(index, offset in the group, numel, shape) of every parameter of the group, in torch's parameter order."""
+        """(index, offset in the group, numel, shape) of every trained parameter of the group, in torch's parameter order.
+        A non-trainable one (never given a gradient) has no optimizer state, as in torch.optim.AdamW."""
         o = self.owner
         base = o._group_range[self.gid][0]
-        return [(i, o._offsets[id(p)] - base, p.numel(), p.shape) for i, p in enumerate(o._group_params[self.gid])]
+        return [(i, o._offsets[id(p)] - base, p.numel(), p.shape) for i, p in enumerate(o._group_params[self.gid])
+                if id(p) not in o._frozen]
 
     def state_dict(self):
         step = int(self.step_t.item())
@@ -308,14 +343,14 @@ class _FusedAdamW:
     def load_state_dict(self, sd):
         st = sd["state"]
         sl = self._slices()
-        if len(sd["param_groups"]) != 1 or len(sd["param_groups"][0]["params"]) != len(sl):
+        ids = list(sd["param_groups"][0]["params"]) if len(sd["param_groups"]) == 1 else []
+        if len(sd["param_groups"]) != 1 or len(ids) != len(self.owner._group_params[self.gid]):
             raise ValueError("loaded state dict has a different number of parameter groups / parameters")
-        ids = list(sd["param_groups"][0]["params"])
         with torch.no_grad():
             self.exp_avg.zero_(); self.exp_avg_sq.zero_(); self.step_t.zero_()
             steps = set()
-            for (i, off, n, shape), key in zip(sl, ids):
-                e = st.get(key)
+            for i, off, n, shape in sl:
+                e = st.get(ids[i])
                 if e is None:
                     continue
                 if tuple(e["exp_avg"].shape) != tuple(shape):
@@ -365,13 +400,17 @@ class Dreamer(nn.Module):
         Aout = conf.action_dim if conf.actor_dist == "onehot" else 2 * conf.action_dim
         cd, IC = conf.cnn_depth, conf.image_channels
         enc = self.wm.encoder
+        rew = self.wm.decoder.reward
+        self._catreward = isinstance(rew, _SupportHead)
+        S = rew._support.numel() if self._catreward else 1
         # embedding = cat(image part [Ei], vecobs part [Ev]); each part has its own buffer and meets W_pe's column slice
         self.d = SimpleNamespace(D=conf.deter_dim, G=conf.stoch_dim, C=conf.stoch_discrete,
                                  Z=conf.stoch_dim * conf.stoch_discrete, Hd=conf.hidden_dim, E=enc.out_dim,
                                  Ei=enc.encoder_image.out_dim if enc.encoder_image is not None else 0,
                                  Ev=enc.encoder_vecobs.out_dim if enc.encoder_vecobs is not None else 0,
                                  K=conf.vecobs_size, A=conf.action_dim, F=features_dim, cd=cd, IC=IC, Aout=Aout,
-                                 Ap=(Aout + 3) // 4 * 4)   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
+                                 Ap=(Aout + 3) // 4 * 4,   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
+                                 S=S, Sp=(S + 3) // 4 * 4 if self._catreward else 1)   # reward head outputs, their row pitch
         self._image = enc.encoder_image is not None
         # (input size, output size, in channels, out channels) of the four 4x4 stride-2 convolutions of the encoder
         self._enc_geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
@@ -400,14 +439,28 @@ class Dreamer(nn.Module):
             "target": list(self.ac.critic_target.parameters()),
         }
         self._names = {id(p): n for n, p in self.named_parameters()}
+        # non-trainable members of a trained group (the categorical reward head's support) keep their place in the group's
+        # parameter list but are stored after the target critic: outside every range the optimizer, grad clipping and the
+        # data-parallel all-reduce walk
+        self._frozen = {id(p) for g in GROUPS for p in self._group_params[g] if not p.requires_grad}
         off = 0
         self._offsets, self._group_range = {}, {}
+
+        def place(p):
+            nonlocal off
+            self._offsets[id(p)] = off
+            off += (p.numel() + 7) // 8 * 8              # every tensor 16-byte aligned in the fp32 AND the fp16 arena (TMA)
+
         for gname in GROUPS + ("target",):
             start = off
             for p in self._group_params[gname]:
-                self._offsets[id(p)] = off
-                off += (p.numel() + 7) // 8 * 8          # every tensor 16-byte aligned in the fp32 AND the fp16 arena (TMA)
+                if id(p) not in self._frozen:
+                    place(p)
             self._group_range[gname] = (start, off)
+        for g in GROUPS:
+            for p in self._group_params[g]:
+                if id(p) in self._frozen:
+                    place(p)
         self._arena_numel = off
         self._train_numel = self._group_range["critic"][1]
 
@@ -429,7 +482,7 @@ class Dreamer(nn.Module):
                 v = arena[o:o + p.numel()].view(p.shape)
                 v.copy_(p.data)
                 p.data = v
-                if g != "target":
+                if g != "target" and id(p) not in self._frozen:
                     p.grad = garena[o:o + p.numel()].view(p.shape)
         self._arena, self._garena, self._arena_device = arena, garena, dev
         self._sarena = torch.zeros_like(arena)     # tf32-rounded shadow of the arena (GEMM operands)
@@ -460,6 +513,8 @@ class Dreamer(nn.Module):
         g = self._group_slice(gid, self._garena)
         self.ops.scale_by(g, grad_out.reshape(1).to(device=g.device, dtype=g.dtype))
         for p in self._group_params[gid]:
+            if id(p) in self._frozen:
+                continue
             if p.grad is None or p.grad.data_ptr() != self._view(self._garena, p).data_ptr():
                 p.grad = self._view(self._garena, p)
 
@@ -1134,9 +1189,15 @@ class Dreamer(nn.Module):
         lp_img, lp_rew, lp_term = tbv[..., 1], tbv[..., 2], tbv[..., 3]
         nanmean = lambda x: torch.nansum(x) / (~torch.isnan(x)).sum()                # functions.py:150-151
         extra_t = {}
-        for sig in (-1, 1):                                                          # decoders.py:96-101
-            m = torch.sign(obs["reward"]) == sig
-            extra_t[f"logprob_reward{sig}"] = lp_rew * m / m
+        if self._catreward:                                                          # decoders.py:85-92: per support bucket
+            kr = dd.kr.view(T, B, I)[:, :, 0]
+            for i in range(d.S):
+                m = kr == i
+                extra_t[f"logprob_reward{i}"] = lp_rew * m / m
+        else:
+            for sig in (-1, 1):                                                      # decoders.py:96-101
+                m = torch.sign(obs["reward"]) == sig
+                extra_t[f"logprob_reward{sig}"] = lp_rew * m / m
         m = obs["terminal"] > 0                                                      # decoders.py:103-106
         extra_t["logprob_terminal1"] = lp_term * m / m
         if self._image:
@@ -1190,13 +1251,18 @@ class Dreamer(nn.Module):
         dd = self._image_decoder(featN, N, tag, img, I) if self._image else SimpleNamespace(l_img=None)
         # reward / terminal heads (decoders.py:257-319)
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
-        yr, yt = b("head.yr", N, 1), b("head.yt", N, 1)
+        yr, yt = b("head.yr", N, d.Sp)[:, :d.S], b("head.yt", N, 1)     # reward logits: S per row at pitch Sp
         dd.rew, dd.term = self._mlp_saved(rp, tag + "rew", N), self._mlp_saved(tp, tag + "term", N)
         self._mlp_fwd(rp, featN, yr, dd.rew)
         self._mlp_fwd(tp, featN, yt, dd.term)
-        dd.l_rew, dd.dyr, dd.rec_r = b("loss.rew", N), b("head.dyr", N, 1), b("head.rec_r", N)
+        dd.l_rew, dd.dyr, dd.rec_r = b("loss.rew", N), b("head.dyr", N, d.Sp)[:, :d.S], b("head.rec_r", N)
         dd.l_term, dd.dyt, dd.rec_t = b("loss.term", N), b("head.dyt", N, 1), b("head.rec_t", N)
-        ops.scalar_head_loss(0, yr, obs["reward"].reshape(NB), I, dd.l_rew, dd.dyr, dd.rec_r)
+        if self._catreward:                  # decoders.py:338-362; dd.kr: each row's target bucket (logging masks)
+            dd.kr = b("head.kr", N, dtype=torch.int32)
+            ops.support_head(yr, self._raw(self.wm.decoder.reward._support), obs["reward"].reshape(NB), I, dd.rec_r,
+                             dd.l_rew, dd.dyr, dd.kr)
+        else:
+            ops.scalar_head_loss(0, yr, obs["reward"].reshape(NB), I, dd.l_rew, dd.dyr, dd.rec_r)
         ops.scalar_head_loss(1, yt, obs["terminal"].reshape(NB), I, dd.l_term, dd.dyt, dd.rec_t)
         if d.K:                              # vector-observation head (decoders.py:66-69, 290-319)
             vp = self._mlp_params(self.wm.decoder.vecobs.model)
@@ -1497,7 +1563,12 @@ class Dreamer(nn.Module):
         vt, v = b("ac.vt", J * N, 1), b("ac.v", J * N, 1)
         fall16 = dr.feats16.view(J * N, d.F) if dr.feats16 is not None else None
         critic = self._mlp_saved(cp, tag + "critic", J * N)
-        self._mlp_fwd(rp, fall, rew, x16=fall16)
+        if self._catreward:                  # the actor-critic learns from the expected reward (dreamer.py:156, common.py:84)
+            rlog = b("ac.rlog", J * N, d.Sp)[:, :d.S]
+            self._mlp_fwd(rp, fall, rlog, x16=fall16)
+            ops.support_head(rlog, self._raw(self.wm.decoder.reward._support), None, 1, rew)
+        else:
+            self._mlp_fwd(rp, fall, rew, x16=fall16)
         self._mlp_fwd(tp, fall, tlog, x16=fall16)
         self._mlp_fwd(ctp, fall, vt, x16=fall16)
         self._mlp_fwd(cp, fall, v, critic, x16=fall16)

@@ -18,6 +18,7 @@ from . import _native
 
 ACT_NONE, ACT_ELU = 0, 1
 GEMM_TC, GEMM_SIMT = 0, 1
+SUPPORT_MAX = 1024                      # PD_SUPPORT_MAX: the widest categorical reward support pd_support_head takes
 
 
 _cur_dev = getattr(torch._C, "_cuda_getDevice", None) or torch.cuda.current_device    # the raw binding: no lazy-init checks per launch
@@ -359,6 +360,16 @@ class NativeOps:
         assert target.shape[1] == K and dy.shape == (M, K) and loss.numel() == M
         self._ck(self.lib.pd_vec_head_loss(self.h, M, K, _ptr(y), _ld(y), _ptr(target), _ld(target), int(tgt_div),
                                            _ptr(loss), _ptr(dy), _ld(dy), self._s()), "pd_vec_head_loss")
+
+    def support_head(self, y, support, target, tgt_div, rec, loss=None, dy=None, idx=None):
+        """Categorical reward head (pd_support_head): rec[m] = softmax(y[m]) . support; with a target (row m reads
+        target[m / tgt_div]) also loss = logsumexp(y) - y[k*], dy = softmax(y) - onehot(k*) and idx = k* (int32)."""
+        M, S = y.shape
+        assert support.numel() == S and (rec is None or rec.numel() == M)
+        assert idx is None or (idx.dtype == torch.int32 and idx.is_contiguous() and idx.numel() == M)
+        self._ck(self.lib.pd_support_head(self.h, M, S, _ptr(y), _ld(y), _ptr(support), _ptr(target), int(tgt_div),
+                                          _ptr(rec), _ptr(loss), _ptr(dy), _ld(dy) if dy is not None else 0, _ptr(idx),
+                                          self._s()), "pd_support_head")
 
     def wm_loss(self, TB, I, kl_weight, w_img, w_rew, w_term, l_img, l_rew, l_term, l_kl, kl_exact, ent_prior,
                 ent_post, w, tb, l_vec=None, w_vec=0.0):
