@@ -171,7 +171,7 @@ typedef struct pd_rssm_fwd_args {
     int32_t *idx;                              /* [T,BI,G] sampled classes */
     void *ws_wzT16;                            /* in: fp16 [Z,Hd] = z_mlp.weight^T (pd_transpose_to_half) */
     void *ws_za16, *ws_h16, *ws_pin16;         /* workspace fp16 [BI,Hd] [BI,D] [BI,Hd] */
-    unsigned int *ws_barrier;                  /* workspace, 16 words, 8-byte aligned, cleared by the call: [0] barrier counter */
+    unsigned int *ws_barrier;                  /* workspace, 16 words, cleared by the call: [0] barrier counter */
     float *ws_ghpart, *ws_y2part;              /* workspace 4*BI*3D and 4*BI*Hd floats: k-slice partial sums of the recurrent products */
 } pd_rssm_fwd_args;
 int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void* stream);
@@ -253,7 +253,7 @@ int pd_col2im_imgloss_t(pd_handle* h, int NB, int Hin, int Win, int Cc, int k, c
 int pd_bias_act_bwd(pd_handle* h, long M, int N, float* dy, long lddy, const float* y, long ldy,
                     int act, float* db, void* stream);
 /* The ELU backward + bias gradient of the layer BELOW fused into the kernel that produces that layer's output gradient
- * (instead of a separate pd_bias_act_bwd pass over the gradient image; PD_B200_FUSE_ACTBWD=0 composes the two launches):
+ * (instead of a separate pd_bias_act_bwd pass over the gradient image):
  *   pd_gemm_actbwd:      C = (A B^T) .* elu'(dact) in the GEMM epilogue, then dbias[n] += sum_m C[m, n] (Linear / explicit-column deconv dX;
  *                        decoders.py:128-155 backward, autograd of nn.ELU + bias)
  *   pd_conv_gemm_actbwd: the same for pd_conv_gemm mode 1 (ConvTranspose2d input gradient gathered by TMA im2col)

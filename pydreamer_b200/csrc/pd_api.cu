@@ -45,8 +45,6 @@ int pd_create(int device_ordinal, pd_handle** out) {
     h->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
     h->gemm_impl = PD_GEMM_TC;
     h->round_ops = 1;
-    h->fuse_actbwd = 1;
-    if (const char* e7 = getenv("PD_B200_FUSE_ACTBWD")) h->fuse_actbwd = atoi(e7);
     cudaSetDevice(device_ordinal);
     for (int i = 0; i < PD_SCRATCH_SLOTS; ++i) {
         PdScratch& sc = h->scratch[i];
@@ -149,7 +147,7 @@ int pd_gemm_actbwd(pd_handle* h, int M, int N, int K, const float* A, long lda, 
     PD_REQUIRE(h, M > 0 && N > 0 && K > 0 && A && B && C && dact, "pd_gemm_actbwd: bad arguments");
     const bool tma_ok = (lda % 4 == 0) && (ldb % 4 == 0) && (ldc % 4 == 0) && ((((uintptr_t)A) & 15) == 0) &&
                         ((((uintptr_t)B) & 15) == 0) && ((((uintptr_t)C) & 15) == 0) && N >= 8 && K >= 8;
-    if (h->gemm_impl == PD_GEMM_SIMT || !tma_ok || !h->fuse_actbwd) {
+    if (h->gemm_impl == PD_GEMM_SIMT || !tma_ok) {
         int rc = pd_gemm(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, C, ldc, nullptr, nullptr, 0, 1, PD_ACT_NONE, 0, 0, 0, stream);
         if (rc) return rc;
         return pd_bias_act_bwd(h, M, N, C, ldc, dact, lddact, PD_ACT_ELU, dbias, stream);
@@ -170,15 +168,8 @@ int pd_conv_gemm_actbwd(pd_handle* h, int NB, int H, int W, int C, int k, const 
     PD_REQUIRE(h, X && O && Cmat && dact, "pd_conv_gemm_actbwd: bad arguments");
     PdEpilogue e;
     e.C = Cmat; e.ldc = ldc; e.bias = nullptr; e.R = nullptr; e.ldr = 0; e.r_div = 1;
-    e.act = PD_ACT_NONE; e.round_out = 0; e.accumulate = 0; e.c_f16 = 0;
-    e.dact = nullptr; e.lddact = 0;
-    if (!h->fuse_actbwd) {
-        int rc = pd_conv_gemm_launch(h, 1, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
-        if (rc) return rc;
-        const int P = (H - k) / 2 + 1, Q = (W - k) / 2 + 1;
-        return pd_bias_act_bwd(h, (long)NB * P * Q, odim, Cmat, ldc, dact, lddact, PD_ACT_ELU, dbias, stream);
-    }
-    e.round_out = h->round_ops; e.dact = dact; e.lddact = lddact;
+    e.act = PD_ACT_NONE; e.round_out = h->round_ops; e.accumulate = 0; e.c_f16 = 0;
+    e.dact = dact; e.lddact = lddact;
     int rc = pd_conv_gemm_launch(h, 1, NB, H, W, C, k, X, O, ldo, o_mn, odim, e, (cudaStream_t)stream);
     if (rc || !dbias) return rc;
     const int P = (H - k) / 2 + 1, Q = (W - k) / 2 + 1;

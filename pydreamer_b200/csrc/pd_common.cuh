@@ -39,7 +39,6 @@ struct pd_handle {
     void* encode_tiled;       // cuTensorMapEncodeTiled entry point
     void* encode_im2col;      // cuTensorMapEncodeIm2col entry point (lazy)
     int gemm_smem_configured;
-    int fuse_actbwd;          // ELU backward + bias gradient inside the producing GEMM / col2im (PD_B200_FUSE_ACTBWD=0: separate pass)
     int round_ops;            // round tensor-core operands to tf32 (rna) where they are produced
     int k1_configured;        // persistent RSSM kernels: shared-memory opt-in done on THIS handle's device
     int k1_ctas;              // ... and the co-resident grid they launch (one CTA per SM)

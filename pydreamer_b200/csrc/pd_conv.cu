@@ -440,7 +440,7 @@ int pd_col2im_actbwd(pd_handle* h, int NB, int Hin, int Win, int Hout, int Wout,
     PD_REQUIRE(h, col && dact && out && Cc >= 1 && k >= 1 && k <= 6, "pd_col2im_actbwd: bad arguments");
     PD_REQUIRE(h, Hout >= (Hin - 1) * 2 + k && Wout >= (Win - 1) * 2 + k, "pd_col2im_actbwd: output smaller than the fold");
     const long total = (long)NB * Hout * Wout * Cc;
-    const bool fused = h->fuse_actbwd && (Cc % 4) == 0 && (192 % (Cc / 4)) == 0 && (ldcol % 4) == 0 &&
+    const bool fused = (Cc % 4) == 0 && (192 % (Cc / 4)) == 0 && (ldcol % 4) == 0 &&
                        ((((uintptr_t)out) | ((uintptr_t)col) | ((uintptr_t)dact)) & 15) == 0;
     if (!fused) {
         int rc = pd_col2im(h, NB, Hin, Win, Hout, Wout, Cc, k, col, ldcol, nullptr, PD_ACT_NONE, 0, out, (long)Hout * Wout * Cc,

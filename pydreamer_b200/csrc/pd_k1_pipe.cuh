@@ -113,26 +113,6 @@ __device__ __forceinline__ void producer_wait_barrier(const unsigned* ctr, unsig
     asm volatile("fence.proxy.async;" ::: "memory");
 }
 
-// Diagnostic: CTA 0 accumulates the nanoseconds between consecutive laps per phase slot into ws_barrier[2 + 2 * slot]
-// (7 uint64 counters); one clock read per phase, no effect on the result.
-struct PhaseClock {
-    unsigned long long last;
-    unsigned long long* acc;
-    __device__ __forceinline__ static unsigned long long now() {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        return t;
-    }
-    __device__ void start(unsigned* ws) { acc = (unsigned long long*)(ws + 2); last = now(); }
-    __device__ void lap(int slot) {
-        if (blockIdx.x == 0 && threadIdx.x == 0) {
-            const unsigned long long t = now();
-            acc[slot] += t - last;
-            last = t;
-        }
-    }
-};
-
 // Stage layout: MAXT weight tiles, then XB activation boxes (X_BOX bytes apart).
 template <int MAXT, int XB>
 struct Ring {                       // both sides count stages identically: slot = n % NSTAGE, parity = (n / NSTAGE) & 1
@@ -167,7 +147,8 @@ struct Job {
     int kcol0, nkb, x2_from;
     // Grouped weight boxes (ngop > 0): the SAME ntile tiles fetched by a few larger TMA operations instead of one 2 KB box per
     // tile — op o fills tiles gdst[o].. from rows grow[o].. of gmap[o]; g3d[o]: a 3-D map (k, row within gate, gate) whose box
-    // spans all gates (a TMA operation costs about the same for a small box as for a large one).
+    // spans all gates (a TMA operation costs about the same for a small box as for a large one).  produce() reads wmap / row0
+    // only when ngop == 0: a job with grouped boxes may leave them unset (jobs B and C of pd_rssm_fwd3.cu do).
     int ngop;
     const CUtensorMap* gmap[3];
     int grow[3], gdst[3], g3d[3];

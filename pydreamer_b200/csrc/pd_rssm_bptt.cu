@@ -131,8 +131,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
 
     // ================================================= consumer warps =================================================
     unsigned epoch = 0;
-    PhaseClock clk;
-    clk.start(a.ws_barrier);
     // LayerNorm / bias gradient accumulators of the batch-row owners (4 features per thread), kept over all timesteps
     float ag2[4] = {0, 0, 0, 0}, ab2[4] = {0, 0, 0, 0}, ax2[4] = {0, 0, 0, 0};
     float ag1[4] = {0, 0, 0, 0}, ab1[4] = {0, 0, 0, 0}, ax1[4] = {0, 0, 0, 0};
@@ -196,7 +194,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             }
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (1) dpost_t complete
-        clk.lap(0);
 
         // ---------------- P2 (row group x k slice): dpin partials = dpost_t . W_pm
         {
@@ -216,7 +213,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             }
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (2) dpin partials complete
-        clk.lap(1);
 
         // ---------------- P3 (batch-row owners): post_norm LayerNorm+ELU backward -> dy2_t
         if (c < BI) {
@@ -234,7 +230,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             ln_bwd_row(dyv, a.y2 + row * Hd, a.pin + row * Hd, a.ln2_g, a.m2[row], a.r2[row], a.dy2 + row * Hd, ag2, ab2, ax2);
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (3) dy2_t complete
-        clk.lap(2);
 
         // ---------------- P4 (hidden-unit owners): dh = dy2_t . W_ph + dfeat_h + carry ; GRU gate backward -> dgi_t, dgh_t
         {
@@ -272,7 +267,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             }
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (4) dgi_t, dgh_t complete
-        clk.lap(3);
 
         // ---------------- P6/7 (row group x k slice): dh_{t-1} partials = dgh_t . W_hh ; dza partials = dgi_t . W_ih
         {
@@ -303,7 +297,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             }
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (5) partials complete
-        clk.lap(4);
 
         // ---------------- P8 (batch-row owners): in_norm LayerNorm+ELU backward -> dx1_t
         if (c < BI) {
@@ -321,7 +314,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
             ln_bwd_row(dyv, a.x1 + row * Hd, a.za + row * Hd, a.ln1_g, a.m1[row], a.r1[row], a.dx1 + row * Hd, ag1, ab1, ax1);
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (6) dx1_t complete
-        clk.lap(5);
 
         // ---------------- P9 (latent-group owners): dz of my (rows, group) = dx1_t . W_z, kept in smem for P1 of step t-1
         if (t > 0) {
@@ -339,7 +331,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_bwd_kernel(const pd_rssm_bw
                 }
             }
             cons_sync();
-            clk.lap(6);
         }
     }
 

@@ -44,7 +44,7 @@ constexpr int SMEM_BYTES = OFF_GI + 48 * 65 * 4;
 constexpr int KSPLIT = 4;
 
 struct FwdMaps {
-    CUtensorMap wih, whh, wph, wpm;            // fp16 weights, box {64 halfs, 16 rows}
+    CUtensorMap wpm;                           // fp16 W_pm, box {64 halfs, 16 rows} (phase D when C <= 16)
     CUtensorMap za, h;                         // fp16 activations [BI, K], box {64 halfs, 64 rows}
     CUtensorMap pin16;                         // fp16 [BI, Hd], box {64 halfs, 16 rows}
     CUtensorMap pin64;                         // the same matrix, box {64 halfs, 64 rows} (MULTI phase D)
@@ -84,7 +84,7 @@ __device__ void ln_elu_row(float (&v)[4], int N, const float* __restrict__ gamma
 
 template <bool MULTI>
 __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_fwd_args a, const __grid_constant__ FwdMaps maps,
-                                                                 const int KS, const int GW) {
+                                                                 const int KS) {
     constexpr int HS = MULTI ? HB : BROWS;                  // row stride of hcs
     constexpr int DR = MULTI ? 64 : 16;                     // batch rows of one phase-D pass
     extern __shared__ uint8_t smem_raw[];
@@ -127,19 +127,18 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     for (int o = tid; o < nu * BI; o += NT) hcs[(o % nu) * HS + o / nu] = __ldcg(a.hin + (long)(o / nu) * D + u4_0 + o % nu);
     __syncthreads();
 
+    // weight tiles come in grouped boxes (FwdMaps); phase D takes one box per 16-row tile unless its C classes fill two tiles.
+    // Jobs B and C always set ngop > 0 and leave wmap / row0 unset: produce() does not read them then.
     auto job_b = [&]() {
         JobF j; j.ntile = nu > 0 ? 3 : 0; j.nx = 1; j.xmap[0] = &maps.za; j.xmap[1] = &maps.za; j.xrow0 = 0; j.xrows = BROWS; j.xf16 = 1;
         j.kcol0 = 0; j.nkb = j.ntile ? (Hd + KB - 1) / KB : 0; j.x2_from = 1 << 30;
-        for (int i = 0; i < MAXT; ++i) { j.wmap[i] = &maps.wih; j.row0[i] = (i % 3) * D + u4_0; }
-        j.ngop = GW ? 1 : 0; j.gmap[0] = &maps.wih3; j.grow[0] = u4_0; j.gdst[0] = 0; j.g3d[0] = 1;
+        j.ngop = 1; j.gmap[0] = &maps.wih3; j.grow[0] = u4_0; j.gdst[0] = 0; j.g3d[0] = 1;
         return j;
     };
     auto job_c = [&]() {
         JobF j; j.ntile = inC ? 14 : 0; j.nx = 1; j.xmap[0] = &maps.h; j.xmap[1] = &maps.h; j.xrow0 = 0; j.xrows = BROWS; j.xf16 = 1;
         j.kcol0 = ks * kslice; j.nkb = j.ntile ? (kslice + KB - 1) / KB : 0; j.x2_from = 1 << 30;
-        for (int i = 0; i < 12; ++i) { j.wmap[i] = &maps.whh; j.row0[i] = (i / 4) * D + u6_0 + 16 * (i % 4); }   // tile = gate * 4 + i
-        for (int i = 0; i < 2; ++i) { j.wmap[12 + i] = &maps.wph; j.row0[12 + i] = f6_0 + 16 * i; }
-        j.ngop = GW ? 2 : 0;
+        j.ngop = 2;                                                     // tile = gate * 4 + i for W_hh, 12 + i for W_ph
         j.gmap[0] = &maps.whh3; j.grow[0] = u6_0; j.gdst[0] = 0; j.g3d[0] = 1;
         j.gmap[1] = &maps.wph32; j.grow[1] = f6_0; j.gdst[1] = 12; j.g3d[1] = 0;
         return j;
@@ -149,7 +148,7 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
         j.xrow0 = b9_0; j.xrows = DR;
         j.xf16 = 1; j.kcol0 = 0; j.nkb = j.ntile ? (Hd + KB - 1) / KB : 0; j.x2_from = 1 << 30;
         for (int i = 0; i < MAXT; ++i) { j.wmap[i] = &maps.wpm; j.row0[i] = g9 * C + 16 * i; }
-        j.ngop = (GW && j.ntile == 2) ? 1 : 0; j.gmap[0] = &maps.wpm32; j.grow[0] = g9 * C; j.gdst[0] = 0; j.g3d[0] = 0;
+        j.ngop = j.ntile == 2 ? 1 : 0; j.gmap[0] = &maps.wpm32; j.grow[0] = g9 * C; j.gdst[0] = 0; j.g3d[0] = 0;
         return j;
     };
 
@@ -174,8 +173,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
 
     // ================================================= consumer warps =================================================
     unsigned epoch = 0;
-    PhaseClock clk;
-    clk.start(a.ws_barrier);
     // phase C: partial products of my rows over my k slice -> global (gh partials only when want_gh, y2 partials when want_y2)
     auto phase_c = [&](bool want_gh, bool want_y2) {
         const JobF j = job_c();
@@ -220,7 +217,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     grid_barrier(a.ws_barrier, epoch);                                          // (p1)
     phase_c(true, false);                                                       // gh_0 = h_0 . W_hh^T (raw; bias and mask at use)
     grid_barrier(a.ws_barrier, epoch);                                          // (p2)
-    clk.lap(0);
 
     for (int t = 0; t < T; ++t) {
         // ---- phase A (CTA b < BI): x1 = mask * gather(WzT, idx_{t-1}) + b_z + aa_t ; LayerNorm + ELU -> za
@@ -280,7 +276,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             ln_elu_row(v, Hd, a.ln1_g, a.ln1_b, a.eps, a.za + row * Hd, za16 + (long)b * Hd, a.m1 + row, a.r1 + row, sh);
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (1) za complete
-        clk.lap(1);
 
         // ---- phase B (hidden-unit owners): gi = za . W_ih^T, GRU gate math, h' -> feat / hin[t+1] / h16
         {
@@ -350,12 +345,10 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             }
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (2) h' complete
-        clk.lap(2);
 
         // ---- phase C: partials of y2 = h' . W_ph^T and of gh_{t+1} = h' . W_hh^T
         phase_c(t + 1 < T, true);
         grid_barrier(a.ws_barrier, epoch);                                      // (3) partials complete
-        clk.lap(3);
 
         // ---- phase C' (CTA b < BI): y2 = partial sums + b_ph + ea_t ; LayerNorm + ELU -> pin
         for (int b = c; b < BI; b += ASTEP) {
@@ -375,7 +368,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             ln_elu_row(v, Hd, a.ln2_g, a.ln2_b, a.eps, a.pin + row * Hd, pin16 + (long)b * Hd, a.m2 + row, a.r2 + row, sh);
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (4) pin complete
-        clk.lap(4);
 
         // ---- phase D (latent-group owners): logits of group g for my rows, softmax, argmax(p / q) -> post, idx, z
         for (int rc = 0; rc < NDC; ++rc) {
@@ -429,7 +421,6 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             }
         }
         if (t + 1 < T) grid_barrier(a.ws_barrier, epoch);                       // (5) idx_t complete
-        clk.lap(5);
     }
 }
 
@@ -468,10 +459,7 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     FwdMaps maps;
     memset(&maps, 0, sizeof(maps));
     const char* who = "pd_rssm_unroll_fwd";
-    int rc = make_map(h, who, &maps.wih, a->w_ih16, 3L * a->D, a->Hd, 16, true);
-    if (!rc) rc = make_map(h, who, &maps.whh, a->w_hh16, 3L * a->D, a->D, 16, true);
-    if (!rc) rc = make_map(h, who, &maps.wph, a->w_ph16, a->Hd, a->D, 16, true);
-    if (!rc) rc = make_map(h, who, &maps.wpm, a->w_pm16, Z, a->Hd, 16, true);
+    int rc = make_map(h, who, &maps.wpm, a->w_pm16, Z, a->Hd, 16, true);
     if (!rc) rc = make_map(h, who, &maps.za, a->ws_za16, a->BI, a->Hd, BROWS, true);
     if (!rc) rc = make_map(h, who, &maps.h, a->ws_h16, a->BI, a->D, BROWS, true);
     if (!rc) rc = make_map(h, who, &maps.pin16, a->ws_pin16, a->BI, a->Hd, 16, true);
@@ -484,10 +472,8 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     if (cudaMemsetAsync(a->ws_barrier, 0, 16 * sizeof(unsigned), s) != cudaSuccess)
         PD_FAIL(h, PD_ERR_LAUNCH, "pd_rssm_unroll_fwd: memset failed");
     pd_rssm_fwd_args args = *a;
-    const char* gwe = getenv("PD_B200_K1_GROUPED_W");           // grouped weight boxes unless PD_B200_K1_GROUPED_W=0
-    int gwv = (gwe && atoi(gwe) == 0) ? 0 : 1;
     int ksv = KS;
-    void* kargs[] = {(void*)&args, (void*)&maps, (void*)&ksv, (void*)&gwv};
+    void* kargs[] = {(void*)&args, (void*)&maps, (void*)&ksv};
     const void* fn = multi ? (const void*)rssm_unroll_fwd3_kernel<true> : (const void*)rssm_unroll_fwd3_kernel<false>;
     cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(P), dim3(NT), kargs, SMEM_REQ, s);
     if (e != cudaSuccess) PD_FAIL(h, PD_ERR_LAUNCH, "pd_rssm_unroll_fwd: %s", cudaGetErrorString(e));

@@ -37,10 +37,10 @@ def kl_balance_arg(kl_balance):
 
 def _persistent_sms(m, enabled):
     """The shared preamble of Dreamer._persistent_rssm_ok / _persistent_bptt_ok: the SM count a persistent RSSM kernel of
-    module `m` spreads over, or None when it cannot run (switched off, restricted under data parallelism, or neither a GPU
-    nor the reference op table, whose stand-ins assume 148 SMs)."""
+    module `m` spreads over, or None when it cannot run (switched off, or neither a GPU nor the reference op table, whose
+    stand-ins assume 148 SMs)."""
     on_gpu = m._arena.is_cuda
-    if not (enabled and m._dp_allows() and (on_gpu or m.ops.is_reference)):
+    if not (enabled and (on_gpu or m.ops.is_reference)):
         return None
     return torch.cuda.get_device_properties(m._arena.device).multi_processor_count if on_gpu else 148
 
@@ -897,10 +897,8 @@ class Dreamer(nn.Module):
     # (B*I <= 256 rows, ...); PD_B200_PERSISTENT_RSSM=0 selects the chain of 9 launches per timestep instead.
     persistent_rssm = os.environ.get("PD_B200_PERSISTENT_RSSM", "1") != "0"
 
-    # BPTT through the posterior unroll as ONE cooperative kernel (csrc/pd_rssm_bptt.cu): opt-in with PD_B200_PERSISTENT_BPTT=1.
-    # Default is the chain of ~12 launches per timestep: standalone the two take the same 4 ms, but the chain's latency-bound
-    # launches share the SMs with the concurrent imagination branch while a cooperative kernel owns all of them for its whole
-    # duration.
+    # BPTT through the posterior unroll as ONE cooperative kernel (csrc/pd_rssm_bptt.cu): opt-in with PD_B200_PERSISTENT_BPTT=1
+    # (faster than the default chain of ~12 launches per timestep in the Atari and DMC steps on the H100: README, Numbers).
     persistent_bptt = os.environ.get("PD_B200_PERSISTENT_BPTT", "0") != "0"
 
     def _persistent_bptt_ok(self, BI):
@@ -930,12 +928,7 @@ class Dreamer(nn.Module):
 
     def _ov(self, bit):
         # (the eager phase timer of bench.py needs one stream)
-        return bool(self.overlap & bit) and self._arena.is_cuda and self._phase_timer is None and self._dp_allows()
-
-    def _dp_allows(self):
-        # Data-parallel runs use the SAME schedule as one GPU (side-stream branches, persistent RSSM kernels, graph replay):
-        # PD_B200_DP_FEATURES=0 restores a conservative single-stream / per-timestep-chain schedule under data parallelism.
-        return self._dp is None or os.environ.get("PD_B200_DP_FEATURES", "1") != "0"
+        return bool(self.overlap & bit) and self._arena.is_cuda and self._phase_timer is None
 
     def _side(self, k):
         key = (k, torch.cuda.current_stream(self._arena.device).cuda_stream)     # one side stream per (purpose, parent)

@@ -78,7 +78,7 @@ def dreamer_gate(kind, BI, D, Hd, G, C, ops):
 
     me = SimpleNamespace(d=SimpleNamespace(D=D, Hd=Hd, G=G, C=C), _arena=torch.empty(0, device=DEV), ops=ops,
                          persistent_rssm=True, persistent_bptt=True, fp16_forward=True, _k1_wzT=torch.empty(0),
-                         _k1b_w={"w": None}, _dp_allows=lambda: True)
+                         _k1b_w={"w": None})
     fn = Dreamer._persistent_rssm_ok if kind == "fwd" else Dreamer._persistent_bptt_ok
     return fn(me, BI)
 
@@ -299,10 +299,8 @@ FWD_CASES = [
 
 
 @gpu
-@pytest.mark.parametrize("grouped", [1, 0] if not CPU else [1], ids=lambda v: f"grouped_w{v}")
 @pytest.mark.parametrize("T,BI,I,D,Hd,G,C,wscale,open_loop", FWD_CASES)
-def test_persistent_fwd_matches_float64_step_reference(ops, monkeypatch, grouped, T, BI, I, D, Hd, G, C, wscale, open_loop):
-    monkeypatch.setenv("PD_B200_K1_GROUPED_W", str(grouped))     # read by the library at each call
+def test_persistent_fwd_matches_float64_step_reference(ops, T, BI, I, D, Hd, G, C, wscale, open_loop):
     assert dreamer_gate("fwd", BI, D, Hd, G, C, ops), "Dreamer would not hand this accepted shape to the kernel"
     prm = make_params(D, Hd, G, C, wscale=wscale, seed=T + BI + D + G)
     x = make_step_inputs(T, BI, I, D, Hd, G, C, open_loop=open_loop, seed=Hd + C)
