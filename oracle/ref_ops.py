@@ -8,6 +8,11 @@ compares with the reference implementation's autograd).  Only tests/, __graft_en
 bench.py's cpu_baseline leg may import it; the product path never does.
 
 Reference lines each op restates are the ones cited in include/pd_b200.h.
+
+Each method refuses (RuntimeError) the arguments its native entry point refuses with PD_REQUIRE: leading dimensions,
+16-byte alignment, the smallest tensor-core shapes and the row / class / channel / horizon limits of the kernels.  A
+schedule that runs on this table therefore also passes the native host checks.  The persistent-kernel stand-ins take the
+shapes their kernels take on a 148-SM GPU (SMS).
 """
 import math
 
@@ -15,6 +20,26 @@ import torch
 import torch.nn.functional as F
 
 ACT_NONE, ACT_ELU = 0, 1
+SMS = 148                   # SM count the persistent RSSM stand-ins assume (Dreamer's predicates do the same off the GPU)
+
+
+def _require(cond, what):
+    """PD_REQUIRE of the native entry point: the same condition refuses the call here."""
+    if not cond:
+        raise RuntimeError(f"{what} unsupported")
+
+
+def _ld(t):
+    """Row stride (elements) of a 2-D view, as NativeOps passes it."""
+    return t.stride(0) if t.shape[0] > 1 else max(t.stride(0), t.shape[1])
+
+
+def _aligned(t, n=16):
+    return t is None or t.data_ptr() % n == 0
+
+
+def _cdiv(a, b):
+    return -(-a // b)
 
 
 def _act(x, act):
@@ -50,6 +75,11 @@ class RefOps:
     # ------------------------------------------------------------------ gemm
     def gemm(self, A, B, C, *, a_mn=False, b_mn=False, bias=None, res=None, r_div=1, act=ACT_NONE,
              round_out=False, accumulate=False, c_zeroed=False):
+        _require(C.numel() > 0 and (A.shape[0] if a_mn else A.shape[1]) > 0, f"pd_gemm: shape {tuple(C.shape)}")
+        _require(not (accumulate and (bias is not None or res is not None or act != ACT_NONE)),
+                 "pd_gemm: accumulate with bias / residual / activation")
+        _require(not (C.dtype == torch.float16 and (accumulate or res is not None)),
+                 "pd_gemm: an fp16 output accumulating or adding a residual")
         a = A.t() if a_mn else A
         b = B if b_mn else B.t()
         v = a @ b
@@ -66,10 +96,18 @@ class RefOps:
 
     # ------------------------------------------------------------------ rowwise
     def gemm_f16(self, A16, B16, C, *, bias=None, res=None, r_div=1, act=ACT_NONE, round_out=False):
+        (M, N), K = C.shape, A16.shape[1]
+        _require(M > 0 and N >= 8 and K >= 8, f"pd_gemm_f16: shape {M} {N} {K}")
+        _require(_ld(A16) % 8 == 0 and _ld(B16) % 8 == 0, f"pd_gemm_f16: lda {_ld(A16)} ldb {_ld(B16)} (% 8)")
+        _require(_aligned(A16) and _aligned(B16), "pd_gemm_f16: operands not 16-byte aligned")
         return self.gemm(A16.to(C.dtype), B16.to(C.dtype), C, bias=bias, res=res, r_div=r_div, act=act)
 
     def conv_gemm(self, mode, X, k, O, Cmat, *, o_mn=False, bias=None, act=ACT_NONE, round_out=False):
         NB, H, W, C = X.shape
+        _require(mode in (1, 2, 3), f"pd_conv_gemm: mode {mode}")
+        _require(C % 4 == 0 and _aligned(X), f"pd_conv_gemm: C={C} (% 4) / X alignment")
+        _require(_ld(O) % 4 == 0 and _aligned(O), f"pd_conv_gemm: ldo={_ld(O)} (% 4) / operand alignment")
+        _require(_ld(Cmat) % 4 == 0 and _aligned(Cmat), f"pd_conv_gemm: ldc={_ld(Cmat)} (% 4) / output alignment")
         P, Q = (H - k) // 2 + 1, (W - k) // 2 + 1
         pat = X.unfold(1, k, 2).unfold(2, k, 2).permute(0, 1, 2, 4, 5, 3).reshape(NB * P * Q, k * k, C)   # (pixels, tap, c)
         if mode == 1:
@@ -92,6 +130,7 @@ class RefOps:
         dst.copy_(src.to(dst.dtype))
 
     def ln_elu_fwd(self, x, gamma, beta, eps, y, mean, rstd, y16=None):
+        _require(1 <= x.shape[1] <= 1024, f"pd_ln_elu_fwd: N={x.shape[1]} (1..1024)")
         mu = x.mean(-1)
         var = x.var(-1, unbiased=False)
         r = 1.0 / torch.sqrt(var + eps)
@@ -102,6 +141,7 @@ class RefOps:
             y16.copy_(y.to(y16.dtype))
 
     def ln_elu_bwd(self, dy, x, y, gamma, mean, rstd, dx, dgamma, dbeta, dbias=None):
+        _require(1 <= x.shape[1] <= 1024, f"pd_ln_elu_bwd: N={x.shape[1]} (1..1024)")
         g = dy * _elu_grad_from_out(y)
         xh = (x - mean[:, None]) * rstd[:, None]
         dgamma.add_((g * xh).sum(0))
@@ -149,6 +189,10 @@ class RefOps:
         """Torch statement of pd_rssm_unroll_fwd (csrc/pd_rssm_fwd3.cu; rssm.py:21-78, 125-153): the whole posterior
         unroll in one call, fp16 weights, LayerNorm outputs and h rounded to fp16 (they are the tensor-core operands)."""
         T, BI, I, D, Hd, G, C = (int(dims[k]) for k in ("T", "BI", "I", "D", "Hd", "G", "C"))
+        RG = SMS // (4 if D % 256 == 0 else 1)
+        _require(T >= 1 and 1 <= BI <= 256 and I >= 1 and BI % I == 0 and Hd <= 1024 and Hd % 8 == 0 and D % 8 == 0 and
+                 1 <= C <= 32 and 1 <= G <= min(SMS, 256) and _cdiv(D, SMS) <= 16 and _cdiv(D, RG) <= 64 and
+                 _cdiv(Hd, RG) <= 32, f"pd_rssm_unroll_fwd: shape {dict(dims)}")
         B = BI // I
         x1, za, m1, r1, gates, feat, hin, zin = (t[k] for k in ("x1", "za", "m1", "r1", "gates", "feat", "hin", "zin"))
         y2, pin, m2, r2, post, idx = (t[k] for k in ("y2", "pin", "m2", "r2", "post", "idx"))
@@ -204,6 +248,11 @@ class RefOps:
         transposed fp16 weights, same per-step formulas as the chain cat_st_bwd / ln_elu_bwd / gru_bwd of this table."""
         T, BI, D, Hd, G, C = (int(dims[k]) for k in ("T", "BI", "D", "Hd", "G", "C"))
         Z = G * C
+        RG2, RG6 = SMS // (4 if Z % 256 == 0 else 1), SMS // (4 if (3 * D) % 256 == 0 else 1)
+        R = max(1, min(4, SMS // G))
+        _require(T >= 1 and 1 <= BI <= min(64, SMS) and Hd <= 1024 and Hd % 8 == 0 and D % 8 == 0 and Z % 8 == 0 and
+                 1 <= C <= 32 and 1 <= G <= SMS and _cdiv(BI, R) <= 16 and _cdiv(D, SMS) <= 16 and _cdiv(Hd, RG2) <= 32 and
+                 _cdiv(D, RG6) <= 64 and _cdiv(Hd, RG6) <= 32, f"pd_rssm_unroll_bwd: shape {dict(dims)}")
         dt = t["dpost"].dtype
         WpmT, WphT, WhhT, WihT, WzT = (t[k].to(dt) for k in ("w_pmT16", "w_phT16", "w_hhT16", "w_ihT16", "w_zT16"))
         v3 = lambda k, n: t[k].view(T, BI, n)
@@ -249,6 +298,7 @@ class RefOps:
             dzin_next = dx1[s] @ WzT.t()
 
     def cat_sample(self, logits, noise, G, C, z, zmask=None, mask_next=None, idx=None, z16=None):
+        _require(1 <= C <= 32, f"pd_cat_sample: C={C} (<= 32)")
         M = logits.shape[0]
         _, p = _group_softmax(logits, G, C)
         k = (p / noise.reshape(M, G, C)).argmax(-1)
@@ -262,6 +312,7 @@ class RefOps:
             idx.copy_(k.to(idx.dtype))
 
     def cat_st_bwd(self, logits, G, C, dz_a, dz_b, mask_b, extra, rowscale, alpha, dlogits):
+        _require(1 <= C <= 32, f"pd_cat_st_bwd: C={C} (<= 32)")
         M = logits.shape[0]
         _, p = _group_softmax(logits, G, C)
         dz = torch.zeros(M, G * C, dtype=logits.dtype, device=logits.device)
@@ -277,6 +328,7 @@ class RefOps:
         dlogits.copy_(d)
 
     def kl(self, post, prior, idx, mode, balance, G, C, loss_kl, kl_exact, ent_post, ent_prior, dpost, dprior):
+        _require(1 <= C <= 32 and 1 <= G <= 32, f"pd_kl: G={G} C={C} (<= 32)")
         M = post.shape[0]
         lp, p = _group_softmax(post, G, C)
         lq, q = _group_softmax(prior, G, C)
@@ -298,6 +350,7 @@ class RefOps:
     # ------------------------------------------------------------------ conv data movement
     def im2col(self, inp, k, korder, col, round_out=True):
         NB, Hin, Win, Cc = inp.shape
+        _require(Hin >= k and Win >= k, f"pd_im2col: input {Hin}x{Win}, kernel {k}")
         Ho, Wo = (Hin - k) // 2 + 1, (Win - k) // 2 + 1
         # patches[n, oy, ox, kh, kw, c]
         p = inp.unfold(1, k, 2).unfold(2, k, 2)  # (NB, Ho, Wo, C, kh, kw)
@@ -317,12 +370,17 @@ class RefOps:
 
     def col2im(self, col, Hin, Win, k, bias, act, out, round_out=True):
         NB, Hout, Wout, Cc = out.shape
+        sN, sY, sX, sC = out.stride()
+        _require(col.dtype != torch.float16 or (sC == 1 and Cc % 4 == 0 and sN % 4 == 0 and sY % 4 == 0 and sX % 4 == 0 and
+                                                _ld(col) % 4 == 0 and _aligned(out) and _aligned(col, 8) and _aligned(bias)),
+                 f"pd_col2im: fp16 column matrix with Cc={Cc}, strides {out.stride()}")
         v = self._col2im(col.to(out.dtype), NB, Hin, Win, Hout, Wout, Cc, k)            # (fp16 column matrices are summed in fp32)
         if bias is not None:
             v = v + bias
         out.copy_(_act(v, act))
 
     def col2im_imgloss(self, col, NB, Hin, Win, Cc, k, bias, target, tgt_div, dec, diff, loss, csum):
+        _require(1 <= Cc <= 16, f"pd_col2im_imgloss: {Cc} image channels (1..16)")
         Hout, Wout = (Hin - 1) * 2 + k, (Win - 1) * 2 + k
         v = self._col2im(col.to(dec.dtype), NB, Hin, Win, Hout, Wout, Cc, k) + bias  # NHWC
         v = v.permute(0, 3, 1, 2)  # NCHW
@@ -350,6 +408,9 @@ class RefOps:
         return Cmat
 
     def col2im_actbwd(self, col, Hin, Win, k, dact, dbias, out):
+        _require(out.shape[3] >= 1 and 1 <= k <= 6, f"pd_col2im_actbwd: Cc={out.shape[3]} k={k}")
+        _require(out.shape[1] >= (Hin - 1) * 2 + k and out.shape[2] >= (Win - 1) * 2 + k,
+                 "pd_col2im_actbwd: output smaller than the fold")
         self.col2im(col, Hin, Win, k, None, ACT_NONE, out, round_out=False)
         NB, Hout, Wout, Cc = out.shape
         self.bias_act_bwd(out.view(-1, Cc), dact.reshape(-1, Cc), ACT_ELU, dbias)
@@ -376,6 +437,8 @@ class RefOps:
         x.mul_(alpha * (scale.reshape(-1)[0] if scale is not None else 1.0))
 
     def gather_rows(self, idx, W, out):
+        _require(out.shape[1] % 4 == 0 and _ld(W) % 4 == 0 and _ld(out) % 4 == 0 and _aligned(W) and _aligned(out),
+                 f"pd_gather_rows: N={out.shape[1]}, ldw={_ld(W)}, ldo={_ld(out)} (% 4) / alignment")
         out.copy_(W[idx.long().reshape(-1)])
 
     def group_sum(self, x, I, out):
@@ -432,10 +495,12 @@ class RefOps:
         tb[:, 7] = 0
 
     def colmean(self, x, out):
+        _require(1 <= x.shape[1] <= 32, f"pd_colmean: N={x.shape[1]} (1..32)")
         out.copy_(x.mean(0))
 
     # ------------------------------------------------------------------ actor critic
     def gae_critic(self, H, Md, gamma, lam, vt, v, rew, term_logit, term, adv, agae, target, weight, dv, sums):
+        _require(1 <= H <= 127, f"pd_gae_critic: H={H} (1..127)")
         J = H + 1
         vt, v, rew = vt.view(J, Md), v.view(J, Md), rew.view(J, Md)
         tm = torch.sigmoid(term_logit.view(J, Md))
@@ -460,6 +525,7 @@ class RefOps:
 
     def actor_loss_onehot(self, eta, logits, actions, agae, weight, dlogits, sums):
         rows, A = actions.shape
+        _require(1 <= A <= 32, f"pd_actor_loss_onehot: A={A} (<= 32)")
         lg = logits[:, :A]
         lp = lg - lg.logsumexp(-1, keepdim=True)
         p = lp.exp()

@@ -35,6 +35,28 @@ def kl_balance_arg(kl_balance):
     return -1.0 if kl_balance in (0.0, 0.5) else float(kl_balance)
 
 
+LN_MAX = 1024              # widest row pd_ln_elu_fwd / pd_ln_elu_bwd normalise
+CAT_MAX = 32               # most classes per group pd_cat_sample / pd_cat_st_bwd / pd_kl / pd_actor_loss_onehot take
+VEC_HEAD_MAX_K = 4096      # PD_VEC_HEAD_MAX_K: the widest vector observation pd_vec_head_loss takes
+IMG_CHANNELS_MAX = 16      # image channels pd_col2im_imgloss takes
+IMAG_HORIZON_MAX = 127     # pd_gae_critic keeps the H + 1 values of a row in registers, H + 1 <= 128
+
+
+def _check_imag_horizon(H):
+    if H > IMAG_HORIZON_MAX:
+        raise NotImplementedError(f"imag_horizon={H}: the return / advantage kernel takes at most {IMAG_HORIZON_MAX} "
+                                  "imagination steps (pd_gae_critic)")
+
+
+def _fp16_path_ok(m):
+    """Dreamer._fp16_forward_ok of module `m`: the fp16-forward path runs when it is switched on and its fp16 GEMMs
+    (pd_gemm_f16) can take the shape.  They read 16-byte rows at 16-byte offsets, so the row lengths and column offsets
+    D, Hd, Z = G * C and F = D + Z must be multiples of 8 halves, and they contract and produce at least 8 columns
+    (Z % 8 == 0 implies Z >= 8)."""
+    d = m.d
+    return bool(m.fp16_forward) and d.D % 8 == 0 and d.Hd % 8 == 0 and (d.G * d.C) % 8 == 0
+
+
 def _persistent_sms(m, enabled):
     """The shared preamble of Dreamer._persistent_rssm_ok / _persistent_bptt_ok: the SM count a persistent RSSM kernel of
     module `m` spreads over, or None when it cannot run (switched off, or neither a GPU nor the reference op table, whose
@@ -388,6 +410,20 @@ class Dreamer(nn.Module):
         if conf.actor_grad != "reinforce":
             raise NotImplementedError("actor_grad=dynamics asserts upstream at a2c.py:131 (SURVEY.md §0.5); "
                                       "the accelerated path implements reinforce")
+        # hard limits of the kernels (a config past one would otherwise fail partway through its first step)
+        for over, what in ((conf.hidden_dim > LN_MAX, f"hidden_dim={conf.hidden_dim}: the LayerNorm kernels take rows of at most "
+                                                      f"{LN_MAX} (pd_ln_elu_fwd / pd_ln_elu_bwd)"),
+                           (conf.actor_dist == "onehot" and conf.action_dim > CAT_MAX,
+                            f"action_dim={conf.action_dim}: the one-hot actor samples and differentiates at most {CAT_MAX} "
+                            "classes (pd_cat_sample, pd_actor_loss_onehot)"),
+                           (conf.vecobs_size > VEC_HEAD_MAX_K, f"vecobs_size={conf.vecobs_size}: the vector-observation loss "
+                                                               f"takes at most {VEC_HEAD_MAX_K} values (pd_vec_head_loss)"),
+                           (bool(conf.image_encoder) and conf.image_channels > IMG_CHANNELS_MAX,
+                            f"image_channels={conf.image_channels}: the image loss takes at most {IMG_CHANNELS_MAX} channels "
+                            "(pd_col2im_imgloss)")):
+            if over:
+                raise NotImplementedError(what)
+        _check_imag_horizon(conf.imag_horizon)
         self.conf = conf
         self.iwae_samples = conf.iwae_samples
         self.imag_horizon = conf.imag_horizon
@@ -635,7 +671,7 @@ class Dreamer(nn.Module):
             return
         ops = self.ops
         ops.round_copy(self._arena, self._sarena, True)
-        if self.fp16_forward:
+        if self._fp16_forward_ok():
             ops.to_half(self._arena.view(1, -1), self._harena.view(1, -1))
         if self._image:
             enc = self.wm.encoder.encoder_image.model
@@ -739,10 +775,14 @@ class Dreamer(nn.Module):
         ops = self.ops
         rows = x_in.shape[0]
         sv = lambda s, l: s[l][:rows]
+        ops.gemm(dout, sv(saved.y, mp.L - 1) if mp.L else x_in, self._g(mp.out.weight), a_mn=True, b_mn=True, accumulate=True)
+        ops.colsum(dout, self._g(mp.out.bias))
+        if mp.L == 0:                   # a head without hidden layers: one Linear
+            if din is not None:
+                ops.gemm(dout, self._w(mp.out.weight), din, b_mn=True, res=din if din_accum else None)
+            return
         dy = self._buf(f"{self._scratch_ns}mlp.dy", rows, mp.hid)
         dx = self._buf(f"{self._scratch_ns}mlp.dx", rows, mp.hid)
-        ops.gemm(dout, sv(saved.y, mp.L - 1), self._g(mp.out.weight), a_mn=True, b_mn=True, accumulate=True)
-        ops.colsum(dout, self._g(mp.out.bias))
         ops.gemm(dout, self._w(mp.out.weight), dy, b_mn=True)
         for l in reversed(range(mp.L)):
             ops.ln_elu_bwd(dy, sv(saved.x, l), sv(saved.y, l), self._raw(mp.ln[l].weight), sv(saved.m, l), sv(saved.r, l),
@@ -783,6 +823,7 @@ class Dreamer(nn.Module):
         assert "terminal" in obs, "`terminal` required in observation"
         I = int(iwae_samples or self.iwae_samples)
         H = int(imag_horizon or self.imag_horizon)
+        _check_imag_horizon(H)
         T, B = obs["action"].shape[:2]
         self._ensure_arena()
         want_grad = torch.is_grad_enabled()
@@ -916,7 +957,7 @@ class Dreamer(nn.Module):
 
     def _persistent_rssm_ok(self, BI):
         d = self.d
-        P = _persistent_sms(self, self.persistent_rssm and self.fp16_forward and getattr(self, "_k1_wzT", None) is not None)
+        P = _persistent_sms(self, self.persistent_rssm and _fp16_path_ok(self) and getattr(self, "_k1_wzT", None) is not None)
         if P is None:
             return False
         ks = 4 if d.D % 256 == 0 and P >= 4 else 1
@@ -925,6 +966,14 @@ class Dreamer(nn.Module):
         # 256 latent groups (MAXG of csrc/pd_rssm_fwd3.cu)
         return (BI <= 256 and d.Hd <= 1024 and d.Hd % 8 == 0 and d.D % 8 == 0 and d.C <= 32 and d.G <= min(P, 256) and
                 cd(d.D, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32)
+
+    def _fp16_forward_ok(self):
+        return _fp16_path_ok(self)
+
+    def _implicit_conv_ok(self):
+        """The implicit-GEMM convolutions (pd_conv_gemm) run when switched on and every activation they read or write has
+        16-byte rows: channel counts cnn_depth x {1, 2, 4, 8} multiples of 4 floats."""
+        return self.implicit_conv and self.d.cd % 4 == 0
 
     def _ov(self, bit):
         # (the eager phase timer of bench.py needs one stream)
@@ -1011,7 +1060,7 @@ class Dreamer(nn.Module):
             x4 = img.permute(0, 2, 3, 1)
             for li, (_, hout, ci, co) in enumerate(self._enc_geo):
                 act, col = b(f"enc.a{li}", NB * hout * hout, co), None
-                if li > 0 and self.implicit_conv:
+                if li > 0 and self._implicit_conv_ok():
                     ops.conv_gemm(1, x4, 4, self._encw[li], act, bias=self._raw(enc[2 * li].bias), act=ACT_ELU, round_out=True)
                 else:
                     col = b(f"enc.col{li}", NB * hout * hout, 16 * ci)
@@ -1208,7 +1257,7 @@ class Dreamer(nn.Module):
     def _cols_dtype(self, ncols):
         """Column matrices of the transposed convolutions are written once and read once: fp16 halves that traffic.  The GEMM's
         fp16 TMA store needs 16-byte rows (ncols % 8 == 0); the last layer (k*k*3 columns) stays fp32."""
-        return torch.float16 if (self.fp16_forward and self.fp16_cols and ncols % 8 == 0) else torch.float32
+        return torch.float16 if (self._fp16_forward_ok() and self.fp16_cols and ncols % 8 == 0) else torch.float32
 
     def _image_decoder(self, featN, N, tag, img=None, I=1):
         """ConvDecoder forward (decoders.py:111-161) on features (N,F): Linear, then each deconvolution as a GEMM into column
@@ -1402,8 +1451,9 @@ class Dreamer(nn.Module):
         b, G = self._buf, self._g
         enc = self.wm.encoder.encoder_image.model
         geo = self._enc_geo
-        cpad = [(ci + 31) // 32 * 32 if self.implicit_conv else ci for _, _, ci, _ in geo]   # implicit: 32 channels per tap
-        encgw = {li: b(("bwd.gencwp" if self.implicit_conv else "bwd.gencw") + str(li), geo[li][3], 16 * cpad[li])
+        implicit = self._implicit_conv_ok()
+        cpad = [(ci + 31) // 32 * 32 if implicit else ci for _, _, ci, _ in geo]   # implicit: 32 channels per tap
+        encgw = {li: b(("bwd.gencwp" if implicit else "bwd.gencw") + str(li), geo[li][3], 16 * cpad[li])
                  for li in (1, 2, 3)}
         for li in (1, 2, 3):
             ops.fill(encgw[li], 0.0)
@@ -1416,7 +1466,7 @@ class Dreamer(nn.Module):
         for li in (3, 2, 1):                # (the ELU / bias of layers 2..0: done by the col2im that produced their gradient)
             hin_, hout, ci, co = geo[li]
             act_prev = fw.enc_act[li - 1]
-            if self.implicit_conv:
+            if implicit:
                 ops.conv_gemm(3, act_prev.view(NB, hin_, hin_, ci), 4, da, encgw[li])
             else:
                 ops.gemm(da, fw.enc_col[li], encgw[li], a_mn=True, b_mn=True, accumulate=True)
@@ -1444,7 +1494,7 @@ class Dreamer(nn.Module):
         ops.rowscale(dd.csum, w, 1, conf.image_weight)
         ops.colsum(dd.csum, G(dec[8].bias))
         dgeo = self._dec_geo
-        impl = [self.implicit_conv and li in (1, 2) for li in range(4)]   # deconv 2,3: 32-channel-aligned NHWC gradients
+        impl = [self._implicit_conv_ok() and li in (1, 2) for li in range(4)]   # deconv 2,3: 32-channel-aligned NHWC gradients
         copad = [(co + 31) // 32 * 32 if impl[li] else co for li, (_, _, _, _, co) in enumerate(dgeo)]
         gdec = [b(("bwd.gdecwp" if impl[li] else "bwd.gdecw") + str(li), k * k * copad[li], ci)
                 for li, (_, _, k, ci, _) in enumerate(dgeo)]                 # rows (tap, co padded), as self._decw
@@ -1496,7 +1546,7 @@ class Dreamer(nn.Module):
         cell = self.wm.core.cell
         gru = cell.gru.layers[0]
         ap = self._mlp_params(self.ac.actor)
-        f16 = self.fp16_forward
+        f16 = self._fp16_forward_ok()
         dr = SimpleNamespace(alog=b("dream.alog", H, N, d.Ap)[..., :d.Aout], actions=b("dream.actions", H, N, d.A),
                              actor=self._mlp_saved(ap, tag + "actor", H * N),
                              feats16=b("feats16", H + 1, N, d.F, dtype=torch.float16) if f16 else None)

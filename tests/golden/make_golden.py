@@ -1,8 +1,8 @@
 """Generates tests/golden/*.json from the UNMODIFIED reference (jurgisp/pydreamer).
 
 Run with a checkout of the reference:
-    python tests/golden/make_golden.py <reference checkout>
-For each case it (1) builds the reference Dreamer, loads seeded weights, (2) seeds the global RNG and runs
+    python tests/golden/make_golden.py <reference checkout> [fixture name ...]
+(without names every fixture below is written).  For each case it (1) builds the reference Dreamer, loads seeded weights, (2) seeds the global RNG and runs
 training_step + the four backward passes exactly as train.py:171-187 does, (3) re-draws the same RNG stream as
 explicit noise (SURVEY.md App. D) and checks oracle/dreamer_oracle.py reproduces losses, metrics and gradients,
 (4) stores the REFERENCE's numbers as the fixture.  Fixtures hold seeds + expected outputs only."""
@@ -28,6 +28,11 @@ CASES = {
     "tiny_iwae3": dict(preset="tiny", over=dict(iwae_samples=3)),
     "tiny_dmc": dict(preset="tiny_dmc", over={}),
     "tiny_klbal05": dict(preset="tiny", over=dict(kl_balance=0.5, kl_weight=1.0)),
+    # shapes off the multiples of 8 / 4 the tensor-core paths need, and heads without hidden layers
+    "tiny_heads0": dict(preset="tiny", over=dict(reward_decoder_layers=0, terminal_decoder_layers=0)),
+    "tiny_odd_dims": dict(preset="tiny", over=dict(hidden_dim=42, deter_dim=70, stoch_dim=5, stoch_discrete=7, cnn_depth=6,
+                                                   image_channels=1)),
+    "tiny_z2": dict(preset="tiny", over=dict(stoch_dim=1, stoch_discrete=2, batch_length=1, imag_horizon=1)),
 }
 NOISE_SEED, DATA_SEED, WEIGHT_SEED = 4321, 1234, 7
 
@@ -135,8 +140,11 @@ def run_log_case(name, spec):
 
 
 if __name__ == "__main__":
+    wanted = sys.argv[2:]
     for n, sp in (("tiny_onehot_log", CASES["tiny_onehot"]), ("tiny_dmc_log", CASES["tiny_dmc"]),
                   ("tiny_iwae3_log", CASES["tiny_iwae3"])):
-        run_log_case(n, sp)
+        if not wanted or n in wanted:
+            run_log_case(n, sp)
     for n, s in CASES.items():
-        run_case(n, s)
+        if not wanted or n in wanted:
+            run_case(n, s)

@@ -42,6 +42,11 @@ def run_gpu(case, impl, rounding, persistent=False):
 @pytest.mark.parametrize("case", CASES)
 def test_exact_arm_matches_reference_golden(case):
     fx, conf, obs, state, noise, model, losses, out_state, metrics, tensors = run_gpu(case, impl=1, rounding=False)
+    check_exact_arm(fx, conf, model, losses, metrics, tensors)
+
+
+def check_exact_arm(fx, conf, model, losses, metrics, tensors):
+    """The exact arm's step (SIMT fp32 GEMM, no operand rounding) against the reference's committed outputs."""
     for got, want in zip(losses, fx["losses"]):
         assert abs(float(got.detach().reshape(-1)[0]) - want) <= 5e-5 * max(1.0, abs(want)), (got, want)
     for k, want in fx["metrics"].items():

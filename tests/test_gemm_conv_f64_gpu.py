@@ -782,7 +782,7 @@ def test_decoder_layer_backward_matches_autograd(ops, round_out, li, implicit):
 def refused(ops, call):
     """A call the host code must refuse with PD_ERR_ARG before launching anything."""
     if CPU:
-        pytest.skip("host-side argument checks of the native library (the float32 twin checks no limits)")
+        pytest.skip("host-side argument checks and launch counts of the native library")
     n0 = ops.launch_count()
     with pytest.raises(RuntimeError, match=r"failed \(-1\)"):
         call()

@@ -20,9 +20,10 @@ def load_fixture(name):
         return json.load(f)
 
 
-def build_case(name, device="cpu"):
-    """-> (fixture, conf, obs, in_state, noise, state_dict_template_fn)"""
-    fx = load_fixture(name)
+def build_case(name, device="cpu", fx=None):
+    """-> (fixture, conf, obs, in_state, noise).  `fx` (instead of the committed fixture `name`): a dict with the
+    fixture's `preset`, `overrides` and `seeds` keys, for a case that has no reference outputs."""
+    fx = fx or load_fixture(name)
     conf = make_conf(fx["preset"], device=str(device), **fx["overrides"])
     T, B, I = conf.batch_length, conf.batch_size, conf.iwae_samples
     obs = synthetic_batch(conf, seed=fx["seeds"]["data"])
