@@ -339,6 +339,14 @@ int pd_gae_critic(pd_handle* h, int H, int Md, float gamma, float lambda,
                   const float* vt, const float* v, const float* rew, const float* term_logit,
                   float* term, float* adv, float* agae, float* target, float* weight, float* dv,
                   double* sums, void* stream);
+/* The same scan over observed rewards and 0/1 terminals: the world model's auxiliary critic (dreamer.py:347-365,
+ * a2c.py:81-116) on T rows (H = T - 1) of B columns.  vt = critic_target values, v = critic values, rew = rewards,
+ * term = terminals (each [T,B]).  dv [T-1,B] = scale * d loss_critic / d v[:-1] with
+ * loss_critic = mean(0.5 (target - v[:-1])^2 weight); a terminal of 1 gives weight 0 at its row and after, never NaN.
+ * sums[2] (double) += {loss_critic * (T-1) B, sum v[:-1]}, added in a fixed order (bit-identical run to run).
+ * 2 <= T <= 128, B >= 1, every pointer non-NULL, otherwise PD_ERR_ARG before any launch. */
+int pd_gae_critic_obs(pd_handle* h, int T, int B, float gamma, float lambda, const float* vt, const float* v,
+                      const float* rew, const float* term, float scale, float* dv, double* sums, void* stream);
 /* reinforce actor loss, one-hot policy (a2c.py:119-130): rows = H*Md.
  * sums[2] (double) += {sum (loss_policy - eta*ent)*w, sum ent};  dlogits = d mean(.)/d logits. */
 int pd_actor_loss_onehot(pd_handle* h, long rows, int A, float eta, const float* logits, long ldl,

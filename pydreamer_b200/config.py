@@ -85,6 +85,19 @@ PRESETS = {
                                              action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, clip_rewards=None,
                                              reward_decoder_categorical=[((5 * i) % 17 - 8) / 8 for i in range(17)] +
                                              [((3 * i) % 16 - 8) / 8 for i in range(16)])),
+    # the world model's auxiliary critic (aux_critic): a critic of the observed rewards on the posterior features, trained
+    # with the world model
+    "atari_auxcritic": (("atari",), dict(deter_dim=2048, batch_size=50, batch_length=50, aux_critic=True)),
+    "tiny_auxcritic": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                        action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, aux_critic=True)),
+    "tiny_auxcritic_iwae3": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                              action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, iwae_samples=3,
+                                              aux_critic=True)),
+    "tiny_dmc_auxcritic": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                          action_dim=3, batch_size=3, batch_length=4, imag_horizon=3,
+                                          actor_grad="reinforce", aux_critic=True)),
+    "tiny_vector_auxcritic": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
+                                                   batch_size=3, batch_length=4, imag_horizon=3, aux_critic=True)),
 }
 
 

@@ -282,59 +282,101 @@ __device__ __forceinline__ void sums_flush(double v, double* ws, unsigned* ticke
     }
 }
 
-constexpr int MAXJ = 128;
-__global__ void gae_critic_kernel(int H, int Md, float gamma, float lambda, const float* __restrict__ vt,
-                                  const float* __restrict__ v, const float* __restrict__ rew,
-                                  const float* __restrict__ tl, float* __restrict__ term, float* __restrict__ adv,
-                                  float* __restrict__ agae, float* __restrict__ target, float* __restrict__ weight,
-                                  float* __restrict__ dv, double* sums, double* ws, unsigned* ticket) {
-    __shared__ double shd[5][8];
-    double s_lc = 0, s_v00 = 0, s_v0 = 0, s_r = 0, s_r2 = 0;
-    const int m = blockIdx.x * blockDim.x + threadIdx.x;
-    if (m < Md) {
-        float tm[MAXJ];
-        const int J = H + 1;
-        for (int j = 0; j < J; ++j) { tm[j] = pd_sigmoid(tl[(long)j * Md + m]); term[(long)j * Md + m] = tm[j]; }
-        float ag = 0.f;
-        const float inv = 1.f / ((float)H * (float)Md);
-        // reversed scan (a2c.py:94-101)
-        for (int j = H - 1; j >= 0; --j) {
-            float v0 = vt[(long)j * Md + m], v1 = vt[(long)(j + 1) * Md + m];
-            float r1 = rew[(long)(j + 1) * Md + m];
-            float a = -v0 + r1 + gamma * (1.0f - tm[j + 1]) * v1;
-            ag = (j == H - 1) ? a : a + lambda * gamma * (1.0f - tm[j + 1]) * ag;
-            adv[(long)j * Md + m] = a;
-            agae[(long)j * Md + m] = ag;
-            target[(long)j * Md + m] = ag + v0;
-            s_r += r1; s_r2 += (double)r1 * r1;
-        }
-        float cs = 0.f;
-        for (int j = 0; j < H; ++j) {
-            cs += logf(1.0f - tm[j]);                 // (1-terminal0).log().cumsum(0).exp()  a2c.py:108
-            float w = expf(cs);
-            weight[(long)j * Md + m] = w;
-            float val = v[(long)j * Md + m];
-            float d = target[(long)j * Md + m] - val;
-            s_lc += 0.5 * (double)d * d * w;
-            dv[(long)j * Md + m] = -d * w * inv;
-            s_v0 += val;
-            if (j == 0) s_v00 += val;
-        }
-    }
-    // block reduce (double)
-    double vals[5] = {s_lc, s_v00, s_v0, s_r, s_r2};
+// Block-wide fixed-order sums of the NQ per-thread values vals[q], then sums_flush.
+template <int NQ>
+__device__ __forceinline__ void block_sums_flush(const double* vals, double* ws, unsigned* ticket, double* sums) {
+    __shared__ double shd[NQ][8];
     const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
 #pragma unroll
-    for (int q = 0; q < 5; ++q) {
+    for (int q = 0; q < NQ; ++q) {
         double x = vals[q];
         for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
         if (lane == 0) shd[q][wp] = x;
     }
     __syncthreads();
     double x = 0;
-    if (threadIdx.x < 5)
+    if (threadIdx.x < NQ)
         for (int i = 0; i < (int)(blockDim.x >> 5); ++i) x += shd[threadIdx.x][i];
-    sums_flush<5>(x, ws, ticket, sums);
+    sums_flush<NQ>(x, ws, ticket, sums);
+}
+
+constexpr int MAXJ = 128;
+// The per-column recursion of a2c.py:88-116 over J = H + 1 rows of column m: GAE(lambda) from the target critic's values
+// vt, the rewards rew[1:] and the terminals tm[1:] (values in [0, 1], held by the caller), the reality weight
+// exp(cumsum(log(1 - tm[:-1]))) (a terminal of 1 gives log 0 = -inf: weight 0 there and after), and the critic loss
+// 0.5 (target - v)^2 weight with dv = -(target - v) weight coef.  STORE writes adv, agae, target and weight (and reads
+// the targets back from `target`); without it the targets stay in a local array.
+// s += {sum loss, sum v[0], sum v[:-1], sum rew[1:], sum rew[1:]^2}.
+template <bool STORE>
+__device__ __forceinline__ void gae_column(int H, int Md, int m, float gamma, float lambda, const float* __restrict__ vt,
+                                           const float* __restrict__ v, const float* __restrict__ rew, const float* tm,
+                                           float coef, float* __restrict__ adv, float* __restrict__ agae,
+                                           float* __restrict__ target, float* __restrict__ weight, float* __restrict__ dv,
+                                           double (&s)[5]) {
+    float tg[STORE ? 1 : MAXJ];
+    float ag = 0.f;
+    // reversed scan (a2c.py:94-101)
+    for (int j = H - 1; j >= 0; --j) {
+        float v0 = vt[(long)j * Md + m], v1 = vt[(long)(j + 1) * Md + m];
+        float r1 = rew[(long)(j + 1) * Md + m];
+        float a = -v0 + r1 + gamma * (1.0f - tm[j + 1]) * v1;
+        ag = (j == H - 1) ? a : a + lambda * gamma * (1.0f - tm[j + 1]) * ag;
+        if (STORE) {
+            adv[(long)j * Md + m] = a;
+            agae[(long)j * Md + m] = ag;
+            target[(long)j * Md + m] = ag + v0;
+        } else {
+            tg[j] = ag + v0;
+        }
+        s[3] += r1; s[4] += (double)r1 * r1;
+    }
+    float cs = 0.f;
+    for (int j = 0; j < H; ++j) {
+        cs += logf(1.0f - tm[j]);                 // (1-terminal0).log().cumsum(0).exp()  a2c.py:108
+        float w = expf(cs);
+        if (STORE) weight[(long)j * Md + m] = w;
+        float val = v[(long)j * Md + m];
+        float d = (STORE ? target[(long)j * Md + m] : tg[j]) - val;
+        s[0] += 0.5 * (double)d * d * w;
+        dv[(long)j * Md + m] = -d * w * coef;
+        s[2] += val;
+        if (j == 0) s[1] += val;
+    }
+}
+
+__global__ void gae_critic_kernel(int H, int Md, float gamma, float lambda, const float* __restrict__ vt,
+                                  const float* __restrict__ v, const float* __restrict__ rew,
+                                  const float* __restrict__ tl, float* __restrict__ term, float* __restrict__ adv,
+                                  float* __restrict__ agae, float* __restrict__ target, float* __restrict__ weight,
+                                  float* __restrict__ dv, double* sums, double* ws, unsigned* ticket) {
+    double s[5] = {0, 0, 0, 0, 0};               // {loss, v0[0], v0, r1, r1^2}
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m < Md) {
+        float tm[MAXJ];
+        const int J = H + 1;
+        for (int j = 0; j < J; ++j) { tm[j] = pd_sigmoid(tl[(long)j * Md + m]); term[(long)j * Md + m] = tm[j]; }
+        const float inv = 1.f / ((float)H * (float)Md);
+        gae_column<true>(H, Md, m, gamma, lambda, vt, v, rew, tm, inv, adv, agae, target, weight, dv, s);
+    }
+    block_sums_flush<5>(s, ws, ticket, sums);
+}
+
+// The same recursion over observed rewards and 0/1 terminals (the world model's auxiliary critic, dreamer.py:347-365):
+// T = H + 1 rows of B columns, dv = scale * d loss / d v; sums[2] += {sum loss, sum v[:-1]}.
+__global__ void gae_critic_obs_kernel(int H, int Md, float gamma, float lambda, const float* __restrict__ vt,
+                                      const float* __restrict__ v, const float* __restrict__ rew,
+                                      const float* __restrict__ term, float scale, float* __restrict__ dv, double* sums,
+                                      double* ws, unsigned* ticket) {
+    double s[5] = {0, 0, 0, 0, 0};
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m < Md) {
+        float tm[MAXJ];
+        for (int j = 0; j <= H; ++j) tm[j] = term[(long)j * Md + m];
+        const float coef = scale / ((float)H * (float)Md);
+        gae_column<false>(H, Md, m, gamma, lambda, vt, v, rew, tm, coef, nullptr, nullptr, nullptr, nullptr, dv, s);
+    }
+    const double vals[2] = {s[0], s[2]};
+    block_sums_flush<2>(vals, ws, ticket, sums);
 }
 
 __global__ void __launch_bounds__(256)
@@ -624,6 +666,20 @@ int pd_gae_critic(pd_handle* h, int H, int Md, float gamma, float lambda, const 
     gae_critic_kernel<<<grid, 128, 0, S(stream)>>>(H, Md, gamma, lambda, vt, v, rew, term_logit, term, adv, agae, target, weight, dv, sums,
                                                    (double*)ws, tk);
     PD_CHECK_LAUNCH(h, "gae_critic");
+    return PD_OK;
+}
+int pd_gae_critic_obs(pd_handle* h, int T, int B, float gamma, float lambda, const float* vt, const float* v,
+                      const float* rew, const float* term, float scale, float* dv, double* sums, void* stream) {
+    PD_REQUIRE(h, T >= 2 && T <= MAXJ && B >= 1 && vt && v && rew && term && dv && sums,
+               "pd_gae_critic_obs: T=%d (2..%d), B=%d (>= 1) unsupported or a NULL pointer", T, MAXJ, B);
+    const int grid = pd_cdiv(B, 128);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), 2L * grid * 2, 1, &ws, &tk);          // grid x 2 doubles
+    if (rc) return rc;
+    gae_critic_obs_kernel<<<grid, 128, 0, S(stream)>>>(T - 1, B, gamma, lambda, vt, v, rew, term, scale, dv, sums,
+                                                       (double*)ws, tk);
+    PD_CHECK_LAUNCH(h, "gae_critic_obs");
     return PD_OK;
 }
 int pd_actor_loss_onehot(pd_handle* h, long rows, int A, float eta, const float* logits, long ldl, const float* actions,

@@ -40,12 +40,19 @@ CAT_MAX = 32               # most classes per group pd_cat_sample / pd_cat_st_bw
 VEC_HEAD_MAX_K = 4096      # PD_VEC_HEAD_MAX_K: the widest vector observation pd_vec_head_loss takes
 IMG_CHANNELS_MAX = 16      # image channels pd_col2im_imgloss takes
 IMAG_HORIZON_MAX = 127     # pd_gae_critic keeps the H + 1 values of a row in registers, H + 1 <= 128
+AUX_T_MAX = 128            # pd_gae_critic_obs scans the T rows of the replayed sequence with the same bound, 2 <= T
 
 
 def _check_imag_horizon(H):
     if H > IMAG_HORIZON_MAX:
         raise NotImplementedError(f"imag_horizon={H}: the return / advantage kernel takes at most {IMAG_HORIZON_MAX} "
                                   "imagination steps (pd_gae_critic)")
+
+
+def _check_aux_length(T):
+    if not 2 <= T <= AUX_T_MAX:
+        raise NotImplementedError(f"aux_critic with sequences of {T} steps: the auxiliary critic's return scan takes 2 to "
+                                  f"{AUX_T_MAX} (pd_gae_critic_obs)")
 
 
 def _fp16_path_ok(m):
@@ -249,8 +256,6 @@ class _WorldModel(nn.Module):
             raise NotImplementedError("Gaussian latents (stoch_discrete=0) are outside the accelerated path (§8f N4)")
         if conf.gru_layers != 1 or conf.gru_type != "gru":
             raise NotImplementedError("accelerated path covers gru_type=gru, gru_layers=1 (SURVEY.md §2 row 3)")
-        if conf.aux_critic:
-            raise NotImplementedError("aux_critic is outside the accelerated path")
         if conf.stoch_discrete > 32 or conf.stoch_dim > 32:
             raise NotImplementedError("categorical kernels handle <= 32 groups of <= 32 classes")
         self.encoder = _MultiEncoder(conf)
@@ -258,6 +263,9 @@ class _WorldModel(nn.Module):
         self.decoder = _MultiDecoder(features_dim, conf)
         self.core = _RSSMCore(self.encoder.out_dim, conf.action_dim, conf.deter_dim, conf.stoch_dim,
                               conf.stoch_discrete, conf.hidden_dim)
+        # dreamer.py:267-279: the auxiliary critic learns the value of the observed rewards on the posterior features; its
+        # actor is built (state_dict keys) but never trained
+        self.ac_aux = _ActorCritic(features_dim, conf.action_dim, conf.layer_norm, conf.actor_dist) if conf.aux_critic else None
         for m in self.modules():
             _init_weights_tf2(m)
 
@@ -424,6 +432,8 @@ class Dreamer(nn.Module):
             if over:
                 raise NotImplementedError(what)
         _check_imag_horizon(conf.imag_horizon)
+        if conf.aux_critic:
+            _check_aux_length(conf.batch_length)
         self.conf = conf
         self.iwae_samples = conf.iwae_samples
         self.imag_horizon = conf.imag_horizon
@@ -475,10 +485,13 @@ class Dreamer(nn.Module):
             "target": list(self.ac.critic_target.parameters()),
         }
         self._names = {id(p): n for n, p in self.named_parameters()}
-        # non-trainable members of a trained group (the categorical reward head's support) keep their place in the group's
-        # parameter list but are stored after the target critic: outside every range the optimizer, grad clipping and the
-        # data-parallel all-reduce walk
+        # members of a trained group that never receive a gradient (the categorical reward head's support, the auxiliary
+        # critic's target and its actor, whose loss the reference discards) keep their place in the group's parameter list
+        # but are stored after the target critic: outside every range the optimizer, grad clipping and the data-parallel
+        # all-reduce walk, so their .grad stays None and torch.optim.AdamW would keep no state for them either
         self._frozen = {id(p) for g in GROUPS for p in self._group_params[g] if not p.requires_grad}
+        if self.wm.ac_aux is not None:
+            self._frozen |= {id(p) for p in self.wm.ac_aux.actor.parameters()}
         off = 0
         self._offsets, self._group_range = {}, {}
 
@@ -825,12 +838,15 @@ class Dreamer(nn.Module):
         H = int(imag_horizon or self.imag_horizon)
         _check_imag_horizon(H)
         T, B = obs["action"].shape[:2]
+        if self.wm.ac_aux is not None:
+            _check_aux_length(T)
         self._ensure_arena()
         want_grad = torch.is_grad_enabled()
         with torch.no_grad():
             if want_grad:
                 self._note_new_grads()
                 self._sync_target_critic()
+                self._sync_aux_target()
             flags = (bool(do_open_loop), bool(do_image_pred), bool(do_dream_tensors and self.wm.decoder.image is not None))
             if flags[0] and want_grad:
                 raise NotImplementedError("do_open_loop is the evaluation branch (train.py:353-359 runs it under no_grad)")
@@ -922,6 +938,18 @@ class Dreamer(nn.Module):
             self._group_slice("target", self._arena).copy_(self._group_slice("critic", self._arena))
             self._weights_dirty = True
         ac.train_steps += 1
+
+    def _sync_aux_target(self):
+        """a2c.py:76-79 for the world model's auxiliary critic: its own counter and target_interval_aux.  Like the main
+        critic's, the counter advances on steps with gradients only."""
+        aux = self.wm.ac_aux
+        if aux is None:
+            return
+        if aux.train_steps % self.conf.target_interval_aux == 0:
+            for pt, pc in zip(aux.critic_target.parameters(), aux.critic.parameters()):
+                self._raw(pt).copy_(self._raw(pc))
+            self._weights_dirty = True
+        aux.train_steps += 1
 
     # set PD_B200_GRAPHS=0 to launch every kernel from Python instead of replaying a captured CUDA graph
     use_cuda_graph = os.environ.get("PD_B200_GRAPHS", "1") != "0"
@@ -1179,6 +1207,7 @@ class Dreamer(nn.Module):
 
         # ---- image decoder + reward / terminal heads on the posterior features
         fw.dec = dd = self._decode_all(featN, fw.img, obs, N, NB, I, "")
+        aux = self._aux_critic_fwd(obs, fw) if self.wm.ac_aux is not None else None
 
         # ---- KL + loss assembly (dreamer.py:328-379)
         l_kl, kl_exact = b("loss.kl", N), b("loss.klx", N)
@@ -1203,9 +1232,36 @@ class Dreamer(nn.Module):
         if d.K:
             metrics.update(loss_vecobs=means[7])
             tensors.update(loss_vecobs=tbv[..., 7], vecobs_rec=self._sel(dd.yv, T, B, I))
+        loss_model = means[0]
+        if aux is not None:                 # dreamer.py:351-365, 369: loss_model stays the metric, the aux term joins the loss
+            loss_model = loss_model + conf.aux_critic_weight * aux["loss"]
+            metrics.update(loss_critic_aux=aux["loss"], policy_value_aux=aux["value_mean"])
+            tensors.update(policy_value_aux=aux["value"])
         if noise_image_pred is not None:
             self._image_pred(obs, fw, prior, noise_image_pred, metrics, tensors)
-        return dict(loss_model=means[0], out_state=fw.out_state, metrics=metrics, tensors=tensors), fw
+        return dict(loss_model=loss_model, out_state=fw.out_state, metrics=metrics, tensors=tensors), fw
+
+    def _aux_critic_fwd(self, obs, fw):
+        """a2c.py:81-116 for the auxiliary critic (dreamer.py:347-365): the target critic and the critic on the posterior
+        features of importance sample 0 (rows t*B*I + b*I of featN, a strided view), then the return scan over the observed
+        rewards and terminals.  Keeps in fw what _wm_backward reads: the critic's activations and dv = aux_critic_weight *
+        d loss_critic_aux / d value[:-1]."""
+        ops, conf, b = self.ops, self.conf, self._buf
+        T, B, I = fw.T, fw.B, fw.I
+        aux = self.wm.ac_aux
+        cp = self._mlp_params(aux.critic)
+        x = fw.featN[::I]                                          # (T*B, F)
+        vt, v = b("aux.vt", T * B, 1), b("aux.v", T * B, 1)
+        fw.aux_critic = self._mlp_saved(cp, "aux.critic", T * B)
+        self._mlp_fwd(self._mlp_params(aux.critic_target), x, vt)
+        self._mlp_fwd(cp, x, v, fw.aux_critic)
+        fw.aux_dv = b("aux.dv", (T - 1) * B, 1)
+        sums = b("aux.sums", 2, dtype=torch.float64)
+        ops.fill(sums.view(torch.float32), 0.0)
+        ops.gae_critic_obs(T, B, conf.gamma_aux, conf.lambda_gae_aux, vt, v, obs["reward"].reshape(T * B),
+                           obs["terminal"].reshape(T * B), conf.aux_critic_weight, fw.aux_dv, sums)
+        hb = float((T - 1) * B)
+        return dict(loss=(sums[0] / hb).to(torch.float32), value_mean=(sums[1] / hb).to(torch.float32), value=v.view(T, B))
 
     @staticmethod
     def _sel(x, T, B, I):
@@ -1339,6 +1395,10 @@ class Dreamer(nn.Module):
         if d.K:
             ops.rowscale(dd.dyv, w, 1, conf.vecobs_weight)
             self._mlp_bwd(self._mlp_params(self.wm.decoder.vecobs.model), featN, dd.dyv, dd.vec, din=dfeat, din_accum=True)
+        if self.wm.ac_aux is not None:      # auxiliary critic: into the sample-0 rows of the first T-1 steps
+            rows = (T - 1) * B
+            self._mlp_bwd(self._mlp_params(self.wm.ac_aux.critic), featN[::I][:rows], fw.aux_dv, fw.aux_critic,
+                          din=dfeat[::I][:rows], din_accum=True)
 
         # ---- prior branch (batch_prior): dprior = kl_weight * w[n] * dKL/dprior
         dprior = fw.dprior

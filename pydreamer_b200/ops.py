@@ -389,6 +389,13 @@ class NativeOps:
                                         _ptr(term_logit), _ptr(term), _ptr(adv), _ptr(agae), _ptr(target),
                                         _ptr(weight), _ptr(dv), _ptr(sums), self._s()), "pd_gae_critic")
 
+    def gae_critic_obs(self, T, B, gamma, lam, vt, v, rew, term, scale, dv, sums):
+        """The GAE / critic-loss scan over observed rewards and 0/1 terminals (pd_gae_critic_obs): T rows of B columns;
+        dv = scale * d loss_critic / d v[:-1]; sums[0:2] (float64) += {loss_critic * (T-1) B, sum v[:-1]}."""
+        assert sums.dtype == torch.float64 and all(t.is_contiguous() for t in (vt, v, rew, term, dv))
+        self._ck(self.lib.pd_gae_critic_obs(self.h, int(T), int(B), float(gamma), float(lam), _ptr(vt), _ptr(v), _ptr(rew),
+                                            _ptr(term), float(scale), _ptr(dv), _ptr(sums), self._s()), "pd_gae_critic_obs")
+
     def actor_loss_onehot(self, eta, logits, actions, agae, weight, dlogits, sums):
         rows, A = actions.shape
         self._ck(self.lib.pd_actor_loss_onehot(self.h, rows, A, float(eta), _ptr(logits), _ld(logits), _ptr(actions),
