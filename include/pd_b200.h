@@ -82,6 +82,17 @@ int pd_gemm(pd_handle* h, int M, int N, int K,
 int pd_gemm_f16(pd_handle* h, int M, int N, int K, const void* A, long lda, const void* B, long ldb,
                 float* C, long ldc, const float* bias, const float* R, long ldr, int r_div,
                 int act, int round_out, void* stream);
+/* Few-row contraction against a weight in its stored orientation (weight-streaming kernel, split-K summed in a fixed order
+ * inside a thread-block cluster): C[M,N] = sum_k A[m][k] * B[k][n] [+ bias[n]] [+ R[m / r_div, n]] -> act -> (tf32
+ * round).  pd_gemm takes this kernel for every call it accepts with a_mn = 0, b_mn = 1 and no accumulate / fp16 C; the
+ * BPTT input gradients of the posterior unroll (rssm.py:103-116 backward, M = B*I rows) are such calls.
+ * It splits K where pd_gemm's tensor-core kernel does and adds the same partial sums in the same order, so both give the
+ * same bits.  Accepts 1 <= M <= 64, N >= 8, K >= 8, A and B 16-byte aligned with lda, ldb multiples of 4, and shapes that
+ * kernel splits at most 16 ways; anything else is PD_ERR_ARG before any launch.  C is written outright (no pre-clear);
+ * any ldc. */
+int pd_gemm_skinny(pd_handle* h, int M, int N, int K, const float* A, long lda, const float* B, long ldb,
+                   float* C, long ldc, const float* bias, const float* R, long ldr, int r_div,
+                   int act, int round_out, void* stream);
 /* Implicit-GEMM convolution contractions: one operand is gathered on the fly from an NHWC fp32 tensor X[NB,H,W,C] by TMA
  * im2col-mode loads (k x k taps, stride 2, no padding; P,Q = (H-k)/2+1) instead of a materialised im2col matrix.
  *   mode 1: Cmat[NB*P*Q, odim] = im2col(X) * O        O: [odim][k*k*C] (o_mn=0) or [k*k*C][odim] (o_mn=1)

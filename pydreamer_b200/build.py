@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpd_b200.so")
 STAMP = os.path.join(HERE, ".libpd_b200.stamp")
-SOURCES = ["pd_api.cu", "pd_gemm_sm90.cu", "pd_gemm_simt.cu", "pd_rowwise.cu", "pd_conv.cu", "pd_misc.cu",
+SOURCES = ["pd_api.cu", "pd_gemm_sm90.cu", "pd_gemm_skinny.cu", "pd_gemm_simt.cu", "pd_rowwise.cu", "pd_conv.cu", "pd_misc.cu",
            "pd_rssm_fwd3.cu", "pd_rssm_bptt.cu"]
 HEADERS = [os.path.join(CSRC, "pd_common.cuh"), os.path.join(CSRC, "pd_k1_pipe.cuh"), os.path.join(HERE, "..", "include", "pd_b200.h")]
 NVCC_FLAGS = [

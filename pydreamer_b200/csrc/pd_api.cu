@@ -9,6 +9,10 @@ int pd_gemm_simt_launch(pd_handle* h, int M, int N, int K, const float* A, long 
 
 int pd_conv_gemm_launch(pd_handle* h, int mode, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo,
                         int o_mn, int ODIM, const PdEpilogue& epi, cudaStream_t stream);
+bool pd_gemm_skinny_ok(const pd_handle* h, int M, int N, int K, const void* A, long lda, int a_mn, const void* B, long ldb,
+                       int b_mn, const PdEpilogue& e);
+int pd_gemm_skinny_launch(pd_handle* h, int M, int N, int K, const float* A, long lda, const float* B, long ldb,
+                          const PdEpilogue& epi, cudaStream_t stream);
 
 int pd_scratch(pd_handle* h, cudaStream_t stream, long nfloats, int ngroups, float** ws, unsigned** tickets) {
     PD_REQUIRE(h, nfloats <= PD_SCRATCH_FLOATS && ngroups <= PD_SCRATCH_TICKETS,
@@ -111,7 +115,21 @@ int pd_gemm(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_m
                         (!e.c_f16 || ((ldc % 8 == 0) && !e.round_out && ((((uintptr_t)C) & 15) == 0)));
     if (h->gemm_impl == PD_GEMM_SIMT || !tma_ok)
         return pd_gemm_simt_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream);
+    // Few rows against a weight stored [K][N] (the BPTT chain's input gradients): stream the weight, not 128-row tiles.
+    if (pd_gemm_skinny_ok(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e))
+        return pd_gemm_skinny_launch(h, M, N, K, A, lda, B, ldb, e, (cudaStream_t)stream);
     return pd_gemm_tc_launch(h, M, N, K, A, lda, a_mn, B, ldb, b_mn, e, (cudaStream_t)stream, 0);
+}
+
+int pd_gemm_skinny(pd_handle* h, int M, int N, int K, const float* A, long lda, const float* B, long ldb, float* C, long ldc,
+                   const float* bias, const float* R, long ldr, int r_div, int act, int round_out, void* stream) {
+    if (!h) return PD_ERR_ARG;
+    PD_REQUIRE(h, A && B && C, "pd_gemm_skinny: null operand");
+    PdEpilogue e;
+    e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
+    e.act = act; e.round_out = round_out && h->round_ops; e.accumulate = 0; e.c_f16 = 0;
+    e.dact = nullptr; e.lddact = 0;
+    return pd_gemm_skinny_launch(h, M, N, K, A, lda, B, ldb, e, (cudaStream_t)stream);
 }
 
 int pd_conv_gemm(pd_handle* h, int mode, int NB, int H, int W, int C, int k, const float* X, const float* O, long ldo, int o_mn,

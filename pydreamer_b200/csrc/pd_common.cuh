@@ -39,6 +39,7 @@ struct pd_handle {
     void* encode_tiled;       // cuTensorMapEncodeTiled entry point
     void* encode_im2col;      // cuTensorMapEncodeIm2col entry point (lazy)
     int gemm_smem_configured;
+    int skinny_smem_configured;   // pd_gemm_skinny_kernel's shared-memory opt-in done
     int round_ops;            // round tensor-core operands to tf32 (rna) where they are produced
     int k1_configured;        // persistent RSSM kernels: shared-memory opt-in done on THIS handle's device
     int k1_ctas;              // ... and the co-resident grid they launch (one CTA per SM)
@@ -50,6 +51,14 @@ struct pd_handle {
 // The scratch area of `stream` (PD_OK), or an error when the handle has seen more streams than it has areas or the
 // launch needs more than one area holds.
 int pd_scratch(pd_handle* h, cudaStream_t stream, long nfloats, int ngroups, float** ws, unsigned** tickets);
+
+// 2-D tensor map of a row-major matrix (dim0 = the contiguous dimension, rows ld_elems apart), 128-byte swizzle, zero
+// fill out of bounds (pd_gemm_sm90.cu).
+int make_map(pd_handle* h, CUtensorMap* tm, const void* base, uint64_t dim0, uint64_t dim1, uint64_t ld_elems,
+             uint32_t box0, uint32_t box1, int elt_bytes = 4);
+// K splits of a storing dense GEMM of M x N outputs and kb_total 32-k blocks (pd_gemm_sm90.cu); pd_gemm_tf32_kernel and
+// pd_gemm_skinny_kernel both split at these k-blocks.
+int pd_gemm_store_splits(const pd_handle* h, int M, int N, int kb_total);
 
 // Launch wrappers run on the handle's device whatever the caller's current device is (and put it back).
 struct PdDeviceGuard {

@@ -496,9 +496,10 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// 2-D tensor map with 128-byte swizzle: dim0 = contiguous dimension.
+}  // namespace
+
 int make_map(pd_handle* h, CUtensorMap* tm, const void* base, uint64_t dim0, uint64_t dim1, uint64_t ld_elems,
-             uint32_t box0, uint32_t box1, int elt_bytes = 4) {
+             uint32_t box0, uint32_t box1, int elt_bytes) {
     cuuint64_t gdim[2] = {dim0, dim1};
     cuuint64_t gstride[1] = {ld_elems * (uint64_t)elt_bytes};
     cuuint32_t box[2] = {box0, box1};
@@ -511,6 +512,8 @@ int make_map(pd_handle* h, CUtensorMap* tm, const void* base, uint64_t dim0, uin
                                    (unsigned long long)dim0, (unsigned long long)dim1, (unsigned long long)ld_elems);
     return PD_OK;
 }
+
+namespace {
 
 // 3-D view of an MN-major fp32 operand [K rows][MN columns, ld]: (32 columns of a group, k, column group) with strides
 // (ld * 4 B, 128 B), box {32, 32, 4} — in shared memory the same bytes as four 2-D {32, 32} boxes 4096 B apart.  Only the
@@ -585,6 +588,19 @@ int pick_splits(int tiles, int kb_total, int slots, int min_kb) {
     }
     return best;
 }
+
+}  // namespace
+
+// Splits of a storing (not accumulating) dense launch: skinny-M layers (the per-timestep RSSM GEMMs, M = B*I = 50: too few
+// output tiles to pull their weights through more than a handful of SMs) split K over the idle SMs.  pd_gemm_skinny_kernel
+// splits its K at the same k-blocks, so both kernels add the same partial sums in the same order.
+int pd_gemm_store_splits(const pd_handle* h, int M, int N, int kb_total) {
+    const int num_m = pd_cdiv(M, BM), tiles = num_m * pd_cdiv(N, BN);
+    const bool skinny = num_m == 1 && tiles * 2 <= h->num_sms && kb_total >= 8;
+    return skinny ? pick_splits(tiles, kb_total, h->num_sms, 4) : 1;
+}
+
+namespace {
 
 int launch(pd_handle* h, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmA3,
            const CUtensorMap& tmB3, GemmArgs& g, int splits, cudaStream_t stream, const char* name) {
@@ -700,10 +716,8 @@ int pd_gemm_tc_launch(pd_handle* h, int M, int N, int K, const void* A, long lda
         tmC = tmA;
     }
     PD_REQUIRE(h, !epi.dact || (g.tma_store && !epi.c_f16 && !epi.accumulate), "pd_gemm(actbwd): needs a TMA-addressable fp32 C");
-    // Weight gradients (accumulate) and skinny-M layers (the per-timestep RSSM GEMMs, M = B*I = 50: too few output tiles to
-    // pull their weights through more than a handful of SMs) split K over the idle SMs.
-    const int tiles = g.num_m * g.num_n;
-    const bool skinny = g.num_m == 1 && tiles * 2 <= h->num_sms && g.kb_total >= 8;
-    const int splits = (epi.accumulate || skinny) ? pick_splits(tiles, g.kb_total, h->num_sms, epi.accumulate ? 8 : 4) : 1;
+    // Weight gradients (accumulate) and skinny-M layers split K over the idle SMs.
+    const int splits = epi.accumulate ? pick_splits(g.num_m * g.num_n, g.kb_total, h->num_sms, 8)
+                                      : pd_gemm_store_splits(h, M, N, g.kb_total);
     return launch(h, tmA, tmB, tmC, tmA3, tmB3, g, splits, stream, "pd_gemm_tf32_kernel");
 }

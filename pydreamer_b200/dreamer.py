@@ -1424,7 +1424,6 @@ class Dreamer(nn.Module):
         dpin, dza = b("bwd.dpin", T, BI, d.Hd), b("bwd.dza", T, BI, d.Hd)
         dhp, dhc = b("bwd.dhp", T, BI, d.D), b("bwd.dhc", BI, d.D)
         dhin, dzin = b("bwd.dhin", T, BI, d.D), b("bwd.dzin", T, BI, d.Z)
-        skinny = BI <= 128
         done = False
         if self._persistent_bptt_ok(BI):
             try:
@@ -1442,27 +1441,24 @@ class Dreamer(nn.Module):
                 warnings.warn(f"pydreamer_b200: persistent BPTT kernel unavailable ({e}); using the per-timestep chain")
                 self.persistent_bptt = False
         par = self._ov(2) and not done
-        if skinny and not done:                     # the chain's split-K GEMMs reduce into pre-cleared outputs
-            for buf_ in (dpin, dza, dhp, dhin, dzin):
-                ops.fill(buf_, 0.0)
         for t in (() if done else reversed(range(T))):
             nxt = t < T - 1
             ops.cat_st_bwd(post[t], d.G, d.C, dfeat3[t, :, d.D:], dzin[t + 1] if nxt else None,
                            mask[t + 1] if nxt else None, dpost_u[t], w3[t], conf.kl_weight, dpost[t])
-            ops.gemm(dpost[t], W(cell.post_mlp.weight), dpin[t], b_mn=True, c_zeroed=skinny)
+            ops.gemm(dpost[t], W(cell.post_mlp.weight), dpin[t], b_mn=True)
             ops.ln_elu_bwd(dpin[t], y2[t], pin[t], self._raw(cell.post_norm.weight), m2[t], r2[t], dy2[t],
                            G(cell.post_norm.weight), G(cell.post_norm.bias), G(cell.post_mlp_h.bias))
-            ops.gemm(dy2[t], W(cell.post_mlp_h.weight), dhp[t], b_mn=True, res=dfeat3[t, :, :d.D], c_zeroed=skinny)
+            ops.gemm(dy2[t], W(cell.post_mlp_h.weight), dhp[t], b_mn=True, res=dfeat3[t, :, :d.D])
             if par and nxt:
                 self._join(2)                       # dhin[t + 1]
             ops.gru_bwd(dhp[t], dhin[t + 1] if nxt else None, mask[t + 1] if nxt else None, gates[t], hin[t], dgi[t],
                         dgh[t], dhc)
             with self._fork(2) if par else contextlib.nullcontext():
-                ops.gemm(dgh[t], W(gru.weight_hh), dhin[t], b_mn=True, res=dhc, c_zeroed=skinny)
-            ops.gemm(dgi[t], W(gru.weight_ih), dza[t], b_mn=True, c_zeroed=skinny)
+                ops.gemm(dgh[t], W(gru.weight_hh), dhin[t], b_mn=True, res=dhc)
+            ops.gemm(dgi[t], W(gru.weight_ih), dza[t], b_mn=True)
             ops.ln_elu_bwd(dza[t], x1[t], za[t], self._raw(cell.in_norm.weight), m1[t], r1[t], dx1[t],
                            G(cell.in_norm.weight), G(cell.in_norm.bias), G(cell.z_mlp.bias))
-            ops.gemm(dx1[t], W(cell.z_mlp.weight), dzin[t], b_mn=True, c_zeroed=skinny)
+            ops.gemm(dx1[t], W(cell.z_mlp.weight), dzin[t], b_mn=True)
         if par:
             self._join(2)
         # batched weight gradients over all T*BI rows
