@@ -212,6 +212,54 @@ __device__ __forceinline__ void wg_wait(float (&acc)[16][4]) {
 #undef PD_ACC64
 #undef PD_D64
 
+// The epilogue of a thread's accumulators, acc[j][x] at row r0 + 8 (x >> 1), column c0 + 8 j + (x & 1): bias and residual
+// unless C accumulates, then, when `finish` (the value is stored, or reduced by TMA), ELU, ELU backward and tf32 rounding.
+// Elements outside C are computed but never stored.  The bias loads of CH n8 blocks are all issued before the first is
+// used, so that their latencies overlap: one load at a time, each waited for by its addition, made the epilogue take
+// longer than the k-loop.  The residual's row offsets (a division) are computed once per tile.  The arithmetic per
+// element is unchanged, so the results are the same bits.
+template <int CH, int NJT>
+__device__ __forceinline__ void epi_apply(const PdEpilogue& e, float (&acc)[NJT][4], int r0, int c0, int M, int N, bool finish) {
+    const bool add = !e.accumulate;
+    const bool in_r[2] = {r0 < M, r0 + 8 < M};
+    const float* rrow[2];
+    const float* drow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        rrow[h] = (add && e.R && in_r[h]) ? e.R + (long)((r0 + 8 * h) / e.r_div) * e.ldr : nullptr;
+        drow[h] = (finish && e.dact && in_r[h]) ? e.dact + (long)(r0 + 8 * h) * e.lddact : nullptr;
+    }
+    const float* bias = add ? e.bias : nullptr;
+#pragma unroll
+    for (int j0 = 0; j0 < NJT; j0 += CH) {
+        float bv[CH][2];
+#pragma unroll
+        for (int j = 0; j < CH; ++j)
+#pragma unroll
+            for (int x = 0; x < 2; ++x) {
+                const int col = c0 + 8 * (j0 + j) + x;
+                bv[j][x] = (bias && col < N) ? __ldg(bias + col) : 0.f;
+            }
+#pragma unroll
+        for (int j = 0; j < CH; ++j)
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
+                const bool in = in_r[x >> 1] && c0 + 8 * (j0 + j) + (x & 1) < N;
+                float v = acc[j0 + j][x];
+                if (add && in) {
+                    if (e.bias) v += bv[j][x & 1];
+                    if (e.R) v += __ldg(rrow[x >> 1] + c0 + 8 * (j0 + j) + (x & 1));
+                }
+                if (finish) {
+                    if (e.act == PD_ACT_ELU) v = pd_elu(v);
+                    if (e.dact && in) v *= pd_elu_grad_from_out(__ldg(drow[x >> 1] + c0 + 8 * (j0 + j) + (x & 1)));
+                    if (e.round_out) v = pd_tf32(v);
+                }
+                acc[j0 + j][x] = v;
+            }
+    }
+}
+
 // 8 consumer warps: two warpgroups of wgmma, a warp owns 16 rows x 128 columns of the output tile.  Warp 8: TMA producer.
 // Warps 9 .. 12: with an MN-major operand, transpose each landed stage to K-major (warp 9 + j takes the 4 KB block j of
 // every MN-major tile) and release it to the consumers through ready[]; otherwise they exit at once.
@@ -405,24 +453,7 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         // ---- epilogue
         const int rbase = m0 + wm, cbase = n0;
         if (rbase >= g.M || cbase >= g.N) continue;                  // warp-uniform: nothing of this slice is real
-#pragma unroll
-        for (int nj = 0; nj < NJ; ++nj)
-#pragma unroll
-            for (int x = 0; x < 4; ++x) {
-                const int row = rbase + g8 + 8 * (x >> 1), col = cbase + nj * 8 + 2 * t4 + (x & 1);
-                float v = acc[nj][x];
-                const bool in = row < g.M && col < g.N;
-                if (!e.accumulate && in) {
-                    if (e.bias) v += __ldg(e.bias + col);
-                    if (e.R) v += __ldg(e.R + (long)(row / e.r_div) * e.ldr + col);
-                }
-                if (g.tma_store || !e.accumulate) {
-                    if (e.act == PD_ACT_ELU) v = pd_elu(v);
-                    if (e.dact && in) v *= pd_elu_grad_from_out(__ldg(e.dact + (long)row * e.lddact + col));
-                    if (e.round_out) v = pd_tf32(v);
-                }
-                acc[nj][x] = v;
-            }
+        epi_apply<4>(e, acc, rbase + g8, cbase + 2 * t4, g.M, g.N, g.tma_store || !e.accumulate);
         if (!g.tma_store) {
             // generic path (C not TMA-addressable: ldc % 4 != 0, e.g. N = 1 / 18 outputs)
 #pragma unroll
