@@ -378,6 +378,30 @@ int pd_image_u8_to_f32(pd_handle* h, long NB, int H, int W, int C, const uint8_t
 int pd_onehot_i64(pd_handle* h, long rows, int A, const int64_t* idx, float* out, void* stream);
 /* y = tanh(x): clip_rewards 'tanh' (functions.py:153-160) */
 int pd_tanh(pd_handle* h, long n, const float* x, float* y, void* stream);
+/* Category ids (NB, P) of id_bytes bytes each (1: uint8, 4: int32, 8: int64) -> fp32 one-hot (NB, C, P)
+ * (preprocessing.py:10-19, 105-110 with C = image_channels).  An id outside [0, C) is a malformed batch: its pixel's C
+ * channels are NaN, and nothing outside `out` is written.  One thread per output element. */
+int pd_image_ids_onehot(pd_handle* h, long NB, int C, int P, const void* ids, int id_bytes, float* out, void* stream);
+
+/* ---- categorical grid images (encoders.py:14-17, 50-60, 99-125; decoders.py:183-254) --------------------------- */
+/* Dense image encoder input rows with reward_input: out[n] = [image[n] (C*P floats, contiguous rows) | reward[n] x P |
+ * terminal[n] x P], row pitch ldo >= (C+2) P.  One thread per output element. */
+int pd_grid_enc_input(pd_handle* h, long NB, int C, int P, const float* image, const float* reward, const float* terminal,
+                      float* out, long ldo, void* stream);
+/* Categorical image loss (CatImageDecoder.loss / training_step) on M rows of C*P logits y in CHW order (channel stride P,
+ * row pitch ldy); row m's target is row m / tgt_div of `target` (one-hot images, pitch ldt).  Per pixel:
+ *   k       = argmax over c of target[c], the first maximum, NaN above everything (torch.argmax);
+ *   loss    = logsumexp(y) - y[k]; with min_prob = m > 0, -log((1 - m) softmax(y)[k] + m / C);
+ *   dy[c]   = d loss / d y[c] (pitch lddy; NULL: not written).
+ * loss[m] (NULL: not written) = the pixel sum.  rec (optional, (M / tgt_div, C, P) contiguous): the decoded image of each
+ * group of tgt_div rows, normalise(logsumexp over the group of normalise(y)) with normalise(x) = x - logsumexp_c(x).
+ * One warp per group, lanes over pixels; every sum is added in a fixed order (bit-identical run to run).
+ * 2 <= C <= PD_CAT_IMAGE_MAX_C, 1 <= P <= PD_CAT_IMAGE_MAX_P, tgt_div >= 1 dividing M, ld* >= C*P, 0 <= min_prob < 1,
+ * otherwise PD_ERR_ARG before any launch. */
+#define PD_CAT_IMAGE_MAX_C 64
+#define PD_CAT_IMAGE_MAX_P 4096
+int pd_cat_image_loss(pd_handle* h, long M, int C, int P, const float* y, long ldy, const float* target, long ldt,
+                      int tgt_div, float min_prob, float* loss, float* dy, long lddy, float* rec, void* stream);
 
 /* ---- optimizer (dreamer.py:60-87, train.py:193-198) ---------------------------------------- */
 /* out += sum x^2 in a fixed summation order (bit-identical on every data-parallel replica); ws: pd_sumsq_ws_floats(h) floats */

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpd_b200.so")
 STAMP = os.path.join(HERE, ".libpd_b200.stamp")
 SOURCES = ["pd_api.cu", "pd_gemm_sm90.cu", "pd_gemm_skinny.cu", "pd_gemm_simt.cu", "pd_rowwise.cu", "pd_conv.cu", "pd_misc.cu",
-           "pd_rssm_fwd3.cu", "pd_rssm_bptt.cu"]
+           "pd_rssm_fwd3.cu", "pd_rssm_bptt.cu", "pd_grid.cu"]
 HEADERS = [os.path.join(CSRC, "pd_common.cuh"), os.path.join(CSRC, "pd_k1_pipe.cuh"), os.path.join(HERE, "..", "include", "pd_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

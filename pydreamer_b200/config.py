@@ -42,6 +42,12 @@ SECTIONS = {
                       image_decoder=None),
     # config/defaults.yaml:244-248 (64x64x3 image + a 27-float vector)
     "minecraft": dict(env_id="Embodied-minecraft_diamond", action_dim=29, vecobs_size=27, clip_rewards="log1p"),
+    # config/defaults.yaml:122-141 (7x7 grid of 4 object categories, one-hot encoded; reward / terminal planes appended to
+    # the encoder input; dense image encoder and categorical image decoder; the map probe)
+    "minigrid": dict(env_id="MiniGrid-MazeS11N-v0", image_key="image", image_size=7, image_channels=4, image_categorical=True,
+                     map_key="map", map_size=11, map_channels=4, map_categorical=True, action_dim=7, reward_input=True,
+                     image_encoder="dense", image_encoder_layers=3, image_decoder="dense", image_decoder_layers=2,
+                     probe_model="map", imag_horizon=1),
 }
 
 # BASELINE.json configs (SURVEY.md §0.4: the shipped YAML differs from BASELINE's wording, so the
@@ -98,6 +104,24 @@ PRESETS = {
                                           actor_grad="reinforce", aux_critic=True)),
     "tiny_vector_auxcritic": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
                                                    batch_size=3, batch_length=4, imag_horizon=3, aux_critic=True)),
+    # categorical grid images (the `minigrid` section) without the map probe: as shipped otherwise (B = 32, T = 48, deter
+    # 2048, H = 1), then tiny shapes: 7x7x4 with reward input, importance samples, the uniform mix of image_decoder_min_prob,
+    # MLPs without hidden layers, a 5x5x3 image without planes (C*H*W = 75 is not a multiple of 4) and a 27-float vector
+    "minigrid": (("minigrid",), dict(probe_model="none")),
+    "tiny_grid": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                      batch_size=3, batch_length=4, imag_horizon=3)),
+    "tiny_grid_iwae3": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                            batch_size=3, batch_length=4, imag_horizon=3, iwae_samples=3)),
+    "tiny_grid_minprob": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                              batch_size=3, batch_length=4, imag_horizon=3, image_decoder_min_prob=0.1)),
+    "tiny_grid_layers0": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                              batch_size=3, batch_length=4, imag_horizon=3, image_encoder_layers=0,
+                                              image_decoder_layers=0)),
+    "tiny_grid_plain": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                            batch_size=3, batch_length=4, imag_horizon=3, reward_input=False, image_size=5,
+                                            image_channels=3)),
+    "tiny_grid_vecobs": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
+                                             batch_size=3, batch_length=4, imag_horizon=3, vecobs_size=27)),
 }
 
 

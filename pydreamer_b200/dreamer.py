@@ -39,6 +39,8 @@ LN_MAX = 1024              # widest row pd_ln_elu_fwd / pd_ln_elu_bwd normalise
 CAT_MAX = 32               # most classes per group pd_cat_sample / pd_cat_st_bwd / pd_kl / pd_actor_loss_onehot take
 VEC_HEAD_MAX_K = 4096      # PD_VEC_HEAD_MAX_K: the widest vector observation pd_vec_head_loss takes
 IMG_CHANNELS_MAX = 16      # image channels pd_col2im_imgloss takes
+CAT_IMAGE_MAX_C = 64       # PD_CAT_IMAGE_MAX_C: the most categories per pixel pd_cat_image_loss takes (2 at least)
+CAT_IMAGE_MAX_P = 4096     # PD_CAT_IMAGE_MAX_P: the most pixels per image pd_cat_image_loss takes
 IMAG_HORIZON_MAX = 127     # pd_gae_critic keeps the H + 1 values of a row in registers, H + 1 <= 128
 AUX_T_MAX = 128            # pd_gae_critic_obs scans the T rows of the replayed sequence with the same bound, 2 <= T
 
@@ -148,27 +150,69 @@ class _ConvEncoder(nn.Module):
 
 
 def _image_modules(conf):
-    """True for the conv image encoder + decoder pair, False for a model without image observations."""
+    """"cnn" for the conv image encoder + decoder pair, "dense" for the dense encoder + categorical decoder pair of grid
+    images, None for a model without image observations."""
     if conf.image_encoder == "cnn" and conf.image_decoder == "cnn":
-        return True
+        return "cnn"
+    if conf.image_encoder == "dense" and conf.image_decoder == "dense":
+        if not conf.image_categorical:
+            raise NotImplementedError("image_decoder=dense is a categorical image decoder (decoders.py:183-254): it takes "
+                                      "the argmax over the channels of the target as the class, so a continuous image "
+                                      "(image_categorical=False) would be trained on a meaningless target")
+        return "dense"
     if not conf.image_encoder and not conf.image_decoder:
-        return False
-    raise NotImplementedError(f"accelerated path covers image_encoder / image_decoder both cnn or both empty, not "
-                              f"{conf.image_encoder!r} / {conf.image_decoder!r} (SURVEY.md §2 rows 4-5)")
+        return None
+    raise NotImplementedError(f"accelerated path covers image_encoder / image_decoder both cnn, both dense or both empty, "
+                              f"not {conf.image_encoder!r} / {conf.image_decoder!r} (SURVEY.md §2 rows 4-5)")
+
+
+class _DenseEncoder(nn.Module):
+    """encoders.py:99-125: Flatten, then max(hidden_layers, 1) x (Linear, LayerNorm, ELU) and Linear + ELU to 256.  The
+    Linear / LayerNorm of hidden layer l sit at model[1 + 3 l] / model[2 + 3 l], the output Linear at model[1 + 3 L]."""
+
+    def __init__(self, in_dim, hidden_layers, layer_norm, hidden_dim=400, out_dim=256):
+        super().__init__()
+        if not layer_norm:
+            raise NotImplementedError("layer_norm=False is outside the accelerated path (SURVEY.md §8f N4)")
+        self.in_dim, self.out_dim, self.hidden_dim = in_dim, out_dim, hidden_dim
+        self.hidden_layers = max(hidden_layers, 1)          # the first hidden layer is always built
+        layers, dim = [nn.Flatten()], in_dim
+        for _ in range(self.hidden_layers):
+            layers += [nn.Linear(dim, hidden_dim), nn.LayerNorm(hidden_dim, eps=1e-3), nn.ELU()]
+            dim = hidden_dim
+        layers += [nn.Linear(dim, out_dim), nn.ELU()]
+        self.model = nn.Sequential(*layers)
+
+
+class _CatImageDecoder(nn.Module):
+    """decoders.py:183-210: hidden_layers x (Linear, LayerNorm, ELU), then Linear to C*H*W logits and Unflatten (one Linear
+    without hidden layers): _mlp_seq's layer indices, with `.model` the Sequential itself."""
+
+    def __init__(self, in_dim, out_shape, hidden_layers, layer_norm, hidden_dim=400):
+        super().__init__()
+        self.in_dim, self.out_dim, self.hidden_dim, self.hidden_layers = in_dim, int(np.prod(out_shape)), hidden_dim, hidden_layers
+        seq = _mlp_seq(in_dim, self.out_dim, hidden_dim, hidden_layers, layer_norm)
+        self.model = nn.Sequential(*seq, nn.Unflatten(-1, tuple(out_shape)))
 
 
 class _MultiEncoder(nn.Module):
-    """encoders.py:10-69: conv embedding of the image and / or an MLP embedding of the vector observation, concatenated
-    image part first."""
+    """encoders.py:10-69: conv or dense embedding of the image and / or an MLP embedding of the vector observation,
+    concatenated image part first.  With reward_input the dense encoder also reads reward and terminal planes."""
 
     def __init__(self, conf):
         super().__init__()
-        if conf.reward_input:
-            raise NotImplementedError("accelerated path covers encoders without reward_input (SURVEY.md §2 row 4)")
         image = _image_modules(conf)
+        if conf.reward_input and image != "dense":
+            raise NotImplementedError("accelerated path covers reward_input with the dense image encoder only "
+                                      "(SURVEY.md §2 row 4)")
         if not image and not conf.vecobs_size:
             raise AssertionError("Either image_encoder or vecobs_size should be set")      # encoders.py:38
-        self.encoder_image = _ConvEncoder(conf.image_channels, conf.cnn_depth) if image else None
+        if image == "dense":
+            chans = conf.image_channels + (2 if conf.reward_input else 0)          # encoders.py:15-18
+            self.encoder_image = _DenseEncoder(conf.image_size * conf.image_size * chans, conf.image_encoder_layers,
+                                               conf.layer_norm)
+        else:
+            self.encoder_image = _ConvEncoder(conf.image_channels, conf.cnn_depth) if image else None
         self.encoder_vecobs = _MLP(conf.vecobs_size, 256, 400, 2, conf.layer_norm) if conf.vecobs_size else None
         self.out_dim = ((self.encoder_image.out_dim if image else 0) +
                         (self.encoder_vecobs.out_dim if conf.vecobs_size else 0))
@@ -190,9 +234,13 @@ class _MultiDecoder(nn.Module):
     def __init__(self, features_dim, conf):
         super().__init__()
         image = _image_modules(conf)
-        if image and conf.image_size != 64:
+        if image == "cnn" and conf.image_size != 64:
             raise NotImplementedError("conv geometry is the reference's 64x64 one (encoders.py:77-90)")
-        self.image = _ConvDecoder(features_dim, conf.image_channels, conf.cnn_depth) if image else None
+        if image == "dense":
+            self.image = _CatImageDecoder(features_dim, (conf.image_channels, conf.image_size, conf.image_size),
+                                          conf.image_decoder_layers, conf.layer_norm)
+        else:
+            self.image = _ConvDecoder(features_dim, conf.image_channels, conf.cnn_depth) if image else None
         if conf.reward_decoder_categorical:         # decoders.py:34-40: the support values are clipped like rewards
             self.reward = _SupportHead(features_dim, _clip_rewards_np(conf.reward_decoder_categorical, conf.clip_rewards),
                                        conf.reward_decoder_layers, conf.layer_norm)
@@ -426,9 +474,15 @@ class Dreamer(nn.Module):
                             "classes (pd_cat_sample, pd_actor_loss_onehot)"),
                            (conf.vecobs_size > VEC_HEAD_MAX_K, f"vecobs_size={conf.vecobs_size}: the vector-observation loss "
                                                                f"takes at most {VEC_HEAD_MAX_K} values (pd_vec_head_loss)"),
-                           (bool(conf.image_encoder) and conf.image_channels > IMG_CHANNELS_MAX,
+                           (conf.image_encoder == "cnn" and conf.image_channels > IMG_CHANNELS_MAX,
                             f"image_channels={conf.image_channels}: the image loss takes at most {IMG_CHANNELS_MAX} channels "
-                            "(pd_col2im_imgloss)")):
+                            "(pd_col2im_imgloss)"),
+                           (conf.image_decoder == "dense" and not 2 <= conf.image_channels <= CAT_IMAGE_MAX_C,
+                            f"image_channels={conf.image_channels}: the categorical image loss takes 2 to {CAT_IMAGE_MAX_C} "
+                            "categories (pd_cat_image_loss)"),
+                           (conf.image_decoder == "dense" and conf.image_size ** 2 > CAT_IMAGE_MAX_P,
+                            f"image_size={conf.image_size}: the categorical image loss takes at most {CAT_IMAGE_MAX_P} "
+                            "pixels (pd_cat_image_loss)")):
             if over:
                 raise NotImplementedError(what)
         _check_imag_horizon(conf.imag_horizon)
@@ -458,6 +512,12 @@ class Dreamer(nn.Module):
                                  Ap=(Aout + 3) // 4 * 4,   # row pitch of the actor outputs: 16-byte rows keep them TMA-addressable
                                  S=S, Sp=(S + 3) // 4 * 4 if self._catreward else 1)   # reward head outputs, their row pitch
         self._image = enc.encoder_image is not None
+        self._dense = isinstance(enc.encoder_image, _DenseEncoder)     # categorical grid images (dense encoder / decoder)
+        self._conv = self._image and not self._dense
+        self._reward_input = bool(conf.reward_input) and self._dense
+        d_ = self.d
+        d_.P = conf.image_size * conf.image_size if self._dense else 0    # pixels of a grid image
+        d_.CP = IC * d_.P                                                   # one-hot image floats (and decoder logits) per row
         # (input size, output size, in channels, out channels) of the four 4x4 stride-2 convolutions of the encoder
         self._enc_geo = ((64, 31, IC, cd), (31, 14, cd, 2 * cd), (14, 6, 2 * cd, 4 * cd), (6, 2, 4 * cd, 8 * cd))
         # (input size, output size, kernel, in channels, out channels) of the four stride-2 deconvolutions of the decoder
@@ -686,7 +746,7 @@ class Dreamer(nn.Module):
         ops.round_copy(self._arena, self._sarena, True)
         if self._fp16_forward_ok():
             ops.to_half(self._arena.view(1, -1), self._harena.view(1, -1))
-        if self._image:
+        if self._conv:
             enc = self.wm.encoder.encoder_image.model
             self._encw = []
             for li, idx in enumerate((0, 2, 4, 6)):
@@ -726,11 +786,13 @@ class Dreamer(nn.Module):
                      (1, 0, 2, 3))
         self._weights_dirty = False
 
-    def _mlp_params(self, mlp):
+    def _mlp_params(self, mlp, off=0):
+        """Layers of an MLP container: hidden layer l's Linear / LayerNorm at model[off + 3 l] / model[off + 3 l + 1], the
+        output Linear at model[off + 3 L] (off = 1 for the dense image encoder, whose model[0] is a Flatten)."""
         seq = mlp.model
         L = mlp.hidden_layers
-        return SimpleNamespace(L=L, lin=[seq[3 * l] for l in range(L)], ln=[seq[3 * l + 1] for l in range(L)],
-                               out=seq[3 * L], hid=mlp.hidden_dim, out_dim=mlp.out_dim, in_dim=mlp.in_dim)
+        return SimpleNamespace(L=L, lin=[seq[off + 3 * l] for l in range(L)], ln=[seq[off + 3 * l + 1] for l in range(L)],
+                               out=seq[off + 3 * L], hid=mlp.hidden_dim, out_dim=mlp.out_dim, in_dim=mlp.in_dim)
 
     # ------------------------------------------------------------------ dense layers
     def _fgemm(self, x, w, out, f16, c_zeroed=False, **kw):
@@ -760,10 +822,11 @@ class Dreamer(nn.Module):
                                m=[b(f"{tag}.m{l}", rows) for l in range(mp.L)],
                                r=[b(f"{tag}.r{l}", rows) for l in range(mp.L)])
 
-    def _mlp_fwd(self, mp, x_in, out, saved=None, row0=0, x16=None):
+    def _mlp_fwd(self, mp, x_in, out, saved=None, row0=0, x16=None, act=ACT_NONE):
         """out[rows, out_dim] = MLP(x_in).  With `saved` (from _mlp_saved) the activations the backward needs are kept in
         its rows [row0, row0+rows); otherwise they go to scratch buffers.
-        x16 (optional, fp16 copy of x_in): run the hidden-layer GEMMs with fp16 operands (forward-only use)."""
+        x16 (optional, fp16 copy of x_in): run the hidden-layer GEMMs with fp16 operands (forward-only use).
+        act: the activation after the output layer (ELU for the dense image encoder)."""
         ops, ns = self.ops, self._scratch_ns
         rows = x_in.shape[0]
         inp, inp16 = x_in, x16
@@ -780,7 +843,7 @@ class Dreamer(nn.Module):
             self._fgemm(inp16 if f16 else inp, mp.lin[l].weight, x, f16, bias=self._raw(mp.lin[l].bias))
             ops.ln_elu_fwd(x, self._raw(mp.ln[l].weight), self._raw(mp.ln[l].bias), 1e-3, y, mean, rstd, y16)
             inp, inp16 = y, y16
-        ops.gemm(inp, self._w(mp.out.weight), out, bias=self._raw(mp.out.bias))     # narrow output layer: fp32 operands
+        ops.gemm(inp, self._w(mp.out.weight), out, bias=self._raw(mp.out.bias), act=act)   # narrow output layer: fp32 operands
 
     def _mlp_bwd(self, mp, x_in, dout, saved, din=None, din_accum=False):
         """Accumulates parameter grads of the MLP from the activations its forward kept in `saved` (first rows of it);
@@ -1078,9 +1141,25 @@ class Dreamer(nn.Module):
         gru = cell.gru.layers[0]
         ea = b("rssm.ea", NB, d.Hd)
         w_pe = self._w(cell.post_mlp_e.weight)         # [Hd, E]: columns [0, Ei) meet the image part, [Ei, E) the vecobs part
-        img = embed = None
+        img = embed = enc_in = denc = None
         acts, cols = [], []
-        if self._image:
+        if self._dense:
+            # ---- dense encoder of grid images (encoders.py:50-60, 99-125): the one-hot image rows, with reward_input
+            # followed by reward and terminal planes; rows of (C+2) H W floats need not be 16-byte multiples, so the first
+            # GEMM (and that layer's weight gradient) take the generic GEMM route
+            ep = self._mlp_params(self.wm.encoder.encoder_image, off=1)
+            img = obs["image"].reshape(NB, d.CP)
+            if self._reward_input:
+                enc_in = b("enc.gin", NB, (d.IC + 2) * d.P)
+                ops.grid_enc_input(img.view(NB, d.IC, d.P, 1), obs["reward"].reshape(NB), obs["terminal"].reshape(NB),
+                                   enc_in)
+            else:
+                enc_in = img
+            embed = b("enc.embed", NB, d.Ei)
+            denc = self._mlp_saved(ep, tag + "denc", NB)
+            self._mlp_fwd(ep, enc_in, embed, denc, act=ACT_ELU)
+            ops.gemm(embed, w_pe[:, :d.Ei], ea)                            # hoisted over T
+        elif self._image:
             # ---- encoder (encoders.py:72-96): im2col -> tensor-core GEMM (+bias+ELU) x4, NHWC activations
             enc = self.wm.encoder.encoder_image.model
             img = obs["image"].reshape(NB, d.IC, 64, 64)
@@ -1125,7 +1204,8 @@ class Dreamer(nn.Module):
         m2, r2 = b("rssm.m2", T, BI), b("rssm.r2", T, BI)
         post = b("rssm.post", T, BI, d.Z)
         idx = b("rssm.idx", T, BI, d.G, dtype=torch.int32)
-        fw = SimpleNamespace(T=T, B=B, I=I, img=img, embed=embed, enc_act=acts, enc_col=cols, vec_in=vec_in,
+        fw = SimpleNamespace(T=T, B=B, I=I, img=img, embed=embed, enc_act=acts, enc_col=cols, enc_in=enc_in, denc=denc,
+                             vec_in=vec_in,
                              vembed=vembed, venc=venc, mask=mask, hin=hin, zin=zin, x1=x1, za=za, m1=m1, r1=r1,
                              gates=gates, y2=y2, pin=pin, m2=m2, r2=r2, post=post, idx=idx)
         head = self._rssm_head(prior=open_loop)     # open loop (rssm.py:52-53): the "posterior" is the prior, no embed
@@ -1225,7 +1305,7 @@ class Dreamer(nn.Module):
         metrics = dict(loss_image=means[1]) if self._image else {}
         metrics.update(loss_reward=means[2], loss_terminal=means[3], loss_model=means[0],
                        loss_kl=means[4], entropy_prior=means[5], entropy_post=means[6])
-        tensors = dict(loss_image=tbv[..., 1], image_rec=self._sel(dd.image, T, B, I)) if self._image else {}
+        tensors = dict(loss_image=tbv[..., 1], image_rec=self._image_out(dd, T, B, I)) if self._image else {}
         tensors.update(loss_reward=tbv[..., 2], reward_rec=self._sel(dd.rec_r, T, B, I), loss_terminal=tbv[..., 3],
                        terminal_rec=self._sel(dd.rec_t, T, B, I), loss_kl=tbv[..., 4], entropy_prior=tbv[..., 5],
                        entropy_post=tbv[..., 6])
@@ -1262,6 +1342,14 @@ class Dreamer(nn.Module):
                            obs["terminal"].reshape(T * B), conf.aux_critic_weight, fw.aux_dv, sums)
         hb = float((T - 1) * B)
         return dict(loss=(sums[0] / hb).to(torch.float32), value_mean=(sums[1] / hb).to(torch.float32), value=v.view(T, B))
+
+    def _image_out(self, dd, T, B, I):
+        """The decoded image (T, B, C, H, W) of a _decode_all namespace: the conv decoder's output averaged over the importance
+        samples, or the categorical decoder's normalised log-probabilities aggregated over them (decoders.py:247-250)."""
+        if self._dense:
+            s = self.conf.image_size
+            return dd.rec.view(T, B, self.d.IC, s, s)
+        return self._sel(dd.image, T, B, I)
 
     @staticmethod
     def _sel(x, T, B, I):
@@ -1300,7 +1388,7 @@ class Dreamer(nn.Module):
         extra_t["logprob_terminal1"] = lp_term * m / m
         if self._image:
             metrics.update(logprob_image=lp_img.mean())
-            tensors.update(logprob_image=lp_img, image_pred=self._sel(dd.image, T, B, I))
+            tensors.update(logprob_image=lp_img, image_pred=self._image_out(dd, T, B, I))
         metrics.update(logprob_reward=lp_rew.mean(), logprob_terminal=lp_term.mean(),
                        **{k: nanmean(v) for k, v in extra_t.items()})
         tensors.update(logprob_reward=lp_rew, logprob_terminal=lp_term, **extra_t,
@@ -1340,13 +1428,29 @@ class Dreamer(nn.Module):
                 ops.col2im(cols, hi, hi, k, bias, ACT_NONE, out.image.permute(0, 2, 3, 1), round_out=False)
         return out
 
+    def _cat_image_decoder(self, featN, N, tag, img, I):
+        """CatImageDecoder.training_step forward (decoders.py:183-254) on features (N,F): the MLP to C*H*W logits, then the
+        per-row loss, its gradient seed and the decoded image of each (t, b) (pd_cat_image_loss against the one-hot target
+        rows `img` (N / I, C*H*W))."""
+        d = self.d
+        b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
+        dp = self._mlp_params(self.wm.decoder.image)
+        out = SimpleNamespace(logits=b("gdec.y", N, d.CP), mlp=self._mlp_saved(dp, tag + "gdec", N))
+        self._mlp_fwd(dp, featN, out.logits, out.mlp)
+        out.l_img, out.diff, out.rec = b("loss.img", N), b("gdec.dy", N, d.CP), b("gdec.rec", N // I, d.CP)
+        self.ops.cat_image_loss(out.logits, d.IC, img, I, self.conf.image_decoder_min_prob, out.l_img, out.diff, out.rec)
+        return out
+
     def _decode_all(self, featN, img, obs, N, NB, I, tag):
         """MultiDecoder.training_step forward (decoders.py:50-108) on features (N,F): the image decoder with its loss and the
         reward / terminal MLP heads with theirs.  Buffers are named `tag + ...` (tag "" = the training pass the backward
         reads); returns the image decoder's namespace extended by the heads'."""
         ops, d = self.ops, self.d
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
-        dd = self._image_decoder(featN, N, tag, img, I) if self._image else SimpleNamespace(l_img=None)
+        if self._dense:
+            dd = self._cat_image_decoder(featN, N, tag, img, I)
+        else:
+            dd = self._image_decoder(featN, N, tag, img, I) if self._image else SimpleNamespace(l_img=None)
         # reward / terminal heads (decoders.py:257-319)
         rp, tp = self._mlp_params(self.wm.decoder.reward.model), self._mlp_params(self.wm.decoder.terminal.model)
         yr, yt = b("head.yr", N, d.Sp)[:, :d.S], b("head.yt", N, 1)     # reward logits: S per row at pitch Sp
@@ -1382,8 +1486,11 @@ class Dreamer(nn.Module):
         gru = cell.gru.layers[0]
         featN, w, dd = fw.featN, fw.w, fw.dec
         dfeat = b("bwd.dfeat", N, d.F)
-        par_w = self._image and self._ov(4)     # image weight gradients leave the dfeat -> BPTT critical path (joined at the end)
-        if self._image:
+        par_w = self._conv and self._ov(4)      # image weight gradients leave the dfeat -> BPTT critical path (joined at the end)
+        if self._dense:                         # categorical image decoder: the first writer of dfeat
+            ops.rowscale(dd.diff, w, 1, conf.image_weight)
+            self._mlp_bwd(self._mlp_params(self.wm.decoder.image), featN, dd.diff, dd.mlp, din=dfeat)
+        elif self._image:
             self._image_decoder_bwd(fw, dfeat, par_w)
 
         # ---- reward / terminal heads (without an image decoder the reward head is the first writer of dfeat)
@@ -1484,7 +1591,14 @@ class Dreamer(nn.Module):
         ops.gemm(daa, obs["action"].reshape(NB, d.A), G(cell.a_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
 
         # ---- encoder backward
-        dea_c = self._image_encoder_bwd(fw, dy2, w_pe[:, :d.Ei]) if self._image else self._dea_c(fw, dy2)
+        if self._dense:
+            dea_c = self._dea_c(fw, dy2)
+            dembed = b("bwd.dembed", NB, d.Ei)
+            # through the encoder's output ELU in the GEMM epilogue (its bias gradient: _mlp_bwd)
+            ops.gemm_actbwd(dea_c, w_pe[:, :d.Ei], dembed, fw.embed, None, b_mn=True)
+            self._mlp_bwd(self._mlp_params(self.wm.encoder.encoder_image, off=1), fw.enc_in, dembed, fw.denc)
+        else:
+            dea_c = self._image_encoder_bwd(fw, dy2, w_pe[:, :d.Ei]) if self._image else self._dea_c(fw, dy2)
         if d.Ev:
             dembed_v = b("bwd.dembed_v", NB, d.Ev)
             ops.gemm(dea_c, w_pe[:, d.Ei:], dembed_v, b_mn=True)
@@ -1710,10 +1824,16 @@ class Dreamer(nn.Module):
         fl[0].copy_(featN[0:BI:I])                                       # states[0, :, 0]
         dr = self._dream(fl, B, Hl, noise_actor, noise_prior, "dl.")
         ac = self._actor_critic(fl, dr, B, Hl, False, "dl.")
-        img = self._image_decoder(fl.view((Hl + 1) * B, d.F), (Hl + 1) * B, "dl.").image
+        rows = (Hl + 1) * B
+        if self._dense:                      # decoders.py:200-203: CatImageDecoder.forward, the raw logits
+            img = self._buf("dl.gdec.y", rows, d.CP)
+            self._mlp_fwd(self._mlp_params(self.wm.decoder.image), fl.view(rows, d.F), img)
+        else:
+            img = self._image_decoder(fl.view(rows, d.F), rows, "dl.").image
+        s = self.conf.image_size
         t = ac["tensors"]
         return dict(action_pred=torch.cat([obs["action"][:1], dr.actions]), reward_pred=ac["rew"], terminal_pred=ac["term"],
-                    image_pred=img.view(T, B, d.IC, 64, 64), value=t["value"], value_target=t["value_target"],
+                    image_pred=img.view(T, B, d.IC, s, s), value=t["value"], value_target=t["value_target"],
                     value_advantage=t["value_advantage"], value_advantage_gae=t["value_advantage_gae"],
                     value_weight=t["value_weight"])
 

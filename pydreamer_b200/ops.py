@@ -425,6 +425,38 @@ class NativeOps:
     def tanh(self, x, y):
         self._ck(self.lib.pd_tanh(self.h, x.numel(), _ptr(x), _ptr(y), self._s()), "pd_tanh")
 
+    def image_ids_onehot(self, ids, out):
+        """Category ids (..., H, W) of uint8 / int32 / int64 -> fp32 one-hot out (..., C, H, W); NaN where an id is
+        outside [0, C) (pd_image_ids_onehot)."""
+        C, H, W = out.shape[-3:]
+        assert ids.shape[-2:] == (H, W) and ids.is_contiguous() and out.is_contiguous()
+        nbytes = {torch.uint8: 1, torch.int32: 4, torch.int64: 8}.get(ids.dtype)
+        if nbytes is None:
+            raise TypeError(f"pd_image_ids_onehot: category ids of dtype {ids.dtype} (uint8, int32 or int64)")
+        self._ck(self.lib.pd_image_ids_onehot(self.h, ids.numel() // (H * W), C, H * W, _ptr(ids), nbytes, _ptr(out),
+                                              self._s()), "pd_image_ids_onehot")
+
+    # ------------------------------------------------------------------ categorical grid images
+    def grid_enc_input(self, image, reward, terminal, out):
+        """out[n] = [image[n] | reward[n] plane | terminal[n] plane] (pd_grid_enc_input); image (NB, C, H, W) contiguous."""
+        NB, C, H, W = image.shape
+        assert image.is_contiguous() and reward.is_contiguous() and terminal.is_contiguous()
+        assert reward.numel() == NB and terminal.numel() == NB and out.shape == (NB, (C + 2) * H * W)
+        self._ck(self.lib.pd_grid_enc_input(self.h, NB, C, H * W, _ptr(image), _ptr(reward), _ptr(terminal), _ptr(out),
+                                            _ld(out), self._s()), "pd_grid_enc_input")
+
+    def cat_image_loss(self, y, C, target, tgt_div, min_prob, loss=None, dy=None, rec=None):
+        """Categorical image loss (pd_cat_image_loss): y (M, C*P) logits, target (M / tgt_div, C*P) one-hot images;
+        loss (M,), dy (M, C*P) and rec (M / tgt_div, C*P) are each optional."""
+        M, CP = y.shape
+        assert CP % C == 0 and target.shape[1] == CP
+        assert dy is None or dy.shape == (M, CP)
+        assert rec is None or (rec.is_contiguous() and rec.numel() == (M // max(tgt_div, 1)) * CP)
+        assert loss is None or (loss.is_contiguous() and loss.numel() == M)
+        self._ck(self.lib.pd_cat_image_loss(self.h, M, C, CP // C, _ptr(y), _ld(y), _ptr(target), _ld(target), int(tgt_div),
+                                            float(min_prob), _ptr(loss), _ptr(dy), _ld(dy) if dy is not None else 0,
+                                            _ptr(rec), self._s()), "pd_cat_image_loss")
+
     # ------------------------------------------------------------------ optimizer
     def sumsq(self, x, out):
         assert x.is_contiguous()

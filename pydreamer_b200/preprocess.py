@@ -3,6 +3,8 @@ path reads.  The raw replay batch (uint8 HWC images, integer actions, raw reward
 123 MB of fp32 per Atari batch — and is converted by three small kernels: SURVEY.md §8(f) row N3.
 
     image    uint8 (T,B,H,W,C)        -> fp32 (T,B,C,H,W) = x/255 - 0.5          preprocessing.py:21-29
+             with image_categorical: category ids (T,B,H,W) of uint8 / int32 / int64 -> fp32 one-hot (T,B,C,H,W),
+             C = image_channels (preprocessing.py:10-19, 105-110); an id outside [0, C) gives NaN channels
     action   int64 (T,B) | fp (T,B,A) -> fp32 one-hot (T,B,A) | as is             preprocessing.py:135-138
     reward   (T,B)                    -> fp32, tanh-clipped if clip_rewards=tanh  preprocessing.py:148-150, functions.py:153-160
     terminal (T,B) -> fp32 ; reset (T,B) bool stays                               preprocessing.py:148
@@ -36,6 +38,13 @@ class GpuPreprocessor:
         img = b.get("image")
         if img is None:
             pass
+        elif conf.image_categorical:
+            C = conf.image_channels
+            H, W = img.shape[-2:]
+            if img.dtype not in (torch.uint8, torch.int32, torch.int64):
+                img = img.to(torch.int64)
+            out["image"] = torch.empty(T, B, C, H, W, device=dev)
+            self.ops.image_ids_onehot(img.contiguous(), out["image"])
         elif img.dtype == torch.uint8:
             H, W, C = img.shape[-3:]
             out["image"] = torch.empty(T, B, C, H, W, device=dev)

@@ -1,6 +1,7 @@
 """Synthetic replay batches in the layout the reference's Preprocessor emits (SURVEY.md §8d).
 
   image    (T,B,C,64,64) fp32 U[-0.5,0.5)          preprocessing.py:21-29 (uint8/255 - 0.5, CHW)
+           with image_categorical: the one-hot (T,B,C,H,W) of the argmax over C of that draw (preprocessing.py:10-19)
   action   (T,B,A)       one-hot fp32 / U[-1,1)     preprocessing.py:135-138, wrappers.py:54-60
   reward   (T,B)         tanh(N(0,1))               clip_rewards: tanh (defaults.yaml:196)
   terminal (T,B)         Bernoulli(0.01) as 0./1.   preprocessing.py:148
@@ -18,6 +19,8 @@ def synthetic_batch(conf, seed=1234, T=None, B=None, first=True, device="cpu", p
     g = torch.Generator().manual_seed(seed)
     A = conf.action_dim
     img = torch.rand(T, B, conf.image_channels, conf.image_size, conf.image_size, generator=g) - 0.5
+    if getattr(conf, "image_categorical", False):        # the one-hot of a uniformly drawn category per pixel
+        img = torch.nn.functional.one_hot(img.argmax(2), conf.image_channels).movedim(-1, 2).float().contiguous()
     if conf.actor_dist == "onehot":
         action = torch.nn.functional.one_hot(torch.randint(0, A, (T, B), generator=g), A).float()
     else:

@@ -31,7 +31,7 @@ def card():
 
 class Arm:
     def __init__(self, preset, dev):
-        from oracle.weights import seeded_state_dict
+        from oracle.grid_oracle import seeded_state_dict      # the weights of oracle/weights.py, grid-aware
         from pydreamer_b200.config import make_conf
         from pydreamer_b200.dreamer import Dreamer
         from pydreamer_b200.replay import synthetic_batch
