@@ -214,10 +214,10 @@ __device__ __forceinline__ void wg_wait(float (&acc)[16][4]) {
 
 // The epilogue of a thread's accumulators, acc[j][x] at row r0 + 8 (x >> 1), column c0 + 8 j + (x & 1): bias and residual
 // unless C accumulates, then, when `finish` (the value is stored, or reduced by TMA), ELU, ELU backward and tf32 rounding.
-// Elements outside C are computed but never stored.  The bias loads of CH n8 blocks are all issued before the first is
-// used, so that their latencies overlap: one load at a time, each waited for by its addition, made the epilogue take
-// longer than the k-loop.  The residual's row offsets (a division) are computed once per tile.  The arithmetic per
-// element is unchanged, so the results are the same bits.
+// Elements outside C are computed but never stored.  The bias, residual and ELU-backward loads of CH n8 blocks are all
+// issued before the first is used, so that their latencies overlap: one load at a time, each waited for by its use, made
+// the epilogue take longer than the k-loop.  The residual's row offsets (a division) are computed once per tile.  The
+// arithmetic per element is unchanged, so the results are the same bits.
 template <int CH, int NJT>
 __device__ __forceinline__ void epi_apply(const PdEpilogue& e, float (&acc)[NJT][4], int r0, int c0, int M, int N, bool finish) {
     const bool add = !e.accumulate;
@@ -232,7 +232,7 @@ __device__ __forceinline__ void epi_apply(const PdEpilogue& e, float (&acc)[NJT]
     const float* bias = add ? e.bias : nullptr;
 #pragma unroll
     for (int j0 = 0; j0 < NJT; j0 += CH) {
-        float bv[CH][2];
+        float bv[CH][2], rv[CH][4], dv[CH][4];
 #pragma unroll
         for (int j = 0; j < CH; ++j)
 #pragma unroll
@@ -244,15 +244,24 @@ __device__ __forceinline__ void epi_apply(const PdEpilogue& e, float (&acc)[NJT]
         for (int j = 0; j < CH; ++j)
 #pragma unroll
             for (int x = 0; x < 4; ++x) {
+                const int col = c0 + 8 * (j0 + j) + (x & 1);
+                const bool in = in_r[x >> 1] && col < N;
+                rv[j][x] = (add && e.R && in) ? __ldg(rrow[x >> 1] + col) : 0.f;
+                dv[j][x] = (finish && e.dact && in) ? __ldg(drow[x >> 1] + col) : 0.f;
+            }
+#pragma unroll
+        for (int j = 0; j < CH; ++j)
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
                 const bool in = in_r[x >> 1] && c0 + 8 * (j0 + j) + (x & 1) < N;
                 float v = acc[j0 + j][x];
                 if (add && in) {
                     if (e.bias) v += bv[j][x & 1];
-                    if (e.R) v += __ldg(rrow[x >> 1] + c0 + 8 * (j0 + j) + (x & 1));
+                    if (e.R) v += rv[j][x];
                 }
                 if (finish) {
                     if (e.act == PD_ACT_ELU) v = pd_elu(v);
-                    if (e.dact && in) v *= pd_elu_grad_from_out(__ldg(drow[x >> 1] + c0 + 8 * (j0 + j) + (x & 1)));
+                    if (e.dact && in) v *= pd_elu_grad_from_out(dv[j][x]);
                     if (e.round_out) v = pd_tf32(v);
                 }
                 acc[j0 + j][x] = v;
@@ -453,7 +462,8 @@ pd_gemm_tf32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         // ---- epilogue
         const int rbase = m0 + wm, cbase = n0;
         if (rbase >= g.M || cbase >= g.N) continue;                  // warp-uniform: nothing of this slice is real
-        epi_apply<4>(e, acc, rbase + g8, cbase + 2 * t4, g.M, g.N, g.tma_store || !e.accumulate);
+        // two n8 blocks per batch of loads: four spill at this kernel's 128 registers and measured slower
+        epi_apply<2>(e, acc, rbase + g8, cbase + 2 * t4, g.M, g.N, g.tma_store || !e.accumulate);
         if (!g.tma_store) {
             // generic path (C not TMA-addressable: ldc % 4 != 0, e.g. N = 1 / 18 outputs)
 #pragma unroll
