@@ -184,6 +184,15 @@ typedef struct pd_rssm_fwd_args {
     void *ws_za16, *ws_h16, *ws_pin16;         /* workspace fp16 [BI,Hd] [BI,D] [BI,Hd] */
     unsigned int *ws_barrier;                  /* workspace, 16 words, cleared by the call: [0] barrier counter */
     float *ws_ghpart, *ws_y2part;              /* workspace 4*BI*3D and 4*BI*Hd floats: k-slice partial sums of the recurrent products */
+    /* Stacked GRU (rnn.py:40-67 GRUCellStack), appended: `layers` = L, 0 or 1 = the single cell above.  For 2 <= L <= 4 layer
+     * l owns the units [l D/L, (l+1) D/L) of h; layer 0 reads za, layer l > 0 the fresh h' of layer l - 1.  w_ih16 / b_ih /
+     * b_hh are then layer 0's ([3D/L, Hd], [3D/L]), w_hh16 is the block-diagonal [3D, D] of the layers' W_hh (row
+     * gate * D + u holds unit u's row of its layer's W_hh in its layer's D/L columns, zeros elsewhere), the arrays below
+     * hold layers 1 .. L-1, and `gates` is laid out [L, T, BI, 4D/L].  Further limits: D/L a multiple of 8,
+     * D/L <= 16 * P (instead of D). */
+    int layers;
+    const void *w_ih16_l[3];                   /* fp16 [3D/L, D/L] of layers 1 .. L-1 */
+    const float *b_ih_l[3], *b_hh_l[3];        /* [3D/L] of layers 1 .. L-1 */
 } pd_rssm_fwd_args;
 int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void* stream);
 

@@ -122,6 +122,21 @@ PRESETS = {
                                             image_channels=3)),
     "tiny_grid_vecobs": (("minigrid",), dict(probe_model="none", deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40,
                                              batch_size=3, batch_length=4, imag_horizon=3, vecobs_size=27)),
+    # a stacked GRU in the RSSM (gru_layers = L: L cells of deter_dim / L units, layer l > 0 reading layer l - 1's new
+    # state): tiny shapes with L = 2, with L = 4 and three importance samples, with the tanh_normal actor, without an image,
+    # and deter 66 in three 22-unit layers (column offsets off the 16-byte multiples); then the Atari benchmark shape
+    "tiny_gru2": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4, action_dim=5,
+                                   batch_size=3, batch_length=4, imag_horizon=3, gru_layers=2)),
+    "tiny_gru4_iwae3": (("atari",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                         action_dim=5, batch_size=3, batch_length=4, imag_horizon=3, iwae_samples=3,
+                                         gru_layers=4)),
+    "tiny_dmc_gru2": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4, action_dim=3,
+                                     batch_size=3, batch_length=4, imag_horizon=3, actor_grad="reinforce", gru_layers=2)),
+    "tiny_vector_gru2": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
+                                              batch_size=3, batch_length=4, imag_horizon=3, gru_layers=2)),
+    "tiny_gru3_odd": (("atari",), dict(deter_dim=66, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4, action_dim=5,
+                                       batch_size=3, batch_length=4, imag_horizon=3, gru_layers=3)),
+    "atari_gru2": (("atari",), dict(deter_dim=2048, batch_size=50, batch_length=50, gru_layers=2)),
 }
 
 

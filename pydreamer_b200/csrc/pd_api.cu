@@ -102,6 +102,9 @@ int pd_gemm(pd_handle* h, int M, int N, int K, const float* A, long lda, int a_m
     PD_REQUIRE(h, M > 0 && N > 0 && K > 0, "pd_gemm: bad shape %d %d %d", M, N, K);
     PD_REQUIRE(h, A && B && C, "pd_gemm: null operand");
     PD_REQUIRE(h, !(accumulate && (bias || R || act)), "pd_gemm: accumulate excludes bias/residual/act");
+    // R may be C itself (C += A.B^T in place, e.g. the BPTT chain's input gradients): every route's epilogue reads R[i, j]
+    // after the contraction, before C[i, j] is written, and no other element's store can overtake that read (each output
+    // tile is read and then stored by the CTA that owns it).  A new epilogue must keep that property.
     PdEpilogue e;
     e.C = C; e.ldc = ldc; e.bias = bias; e.R = R; e.ldr = ldr; e.r_div = r_div > 0 ? r_div : 1;
     e.act = act; e.round_out = round_out && h->round_ops; e.accumulate = accumulate;

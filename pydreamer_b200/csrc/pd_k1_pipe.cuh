@@ -313,9 +313,10 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // row-major [rows, K] matrix as a 2-D tensor map, boxes of 128 bytes x box_rows, 128-byte swizzle, zero OOB fill
-inline int make_map(pd_handle* h, const char* who, CUtensorMap* tm, const void* base, long rows, int K, int box_rows, bool f16) {
+inline int make_map(pd_handle* h, const char* who, CUtensorMap* tm, const void* base, long rows, int K, int box_rows, bool f16,
+                    long ld = 0) {                     // ld: row stride in elements (0: K, a dense matrix)
     cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)K * (f16 ? 2 : 4)};
+    cuuint64_t gstride[1] = {(cuuint64_t)(ld ? ld : K) * (f16 ? 2 : 4)};
     cuuint32_t box[2] = {(cuuint32_t)(f16 ? 64 : 32), (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = ((EncodeTiledFn)h->encode_tiled)(tm, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,

@@ -19,6 +19,13 @@
 // All contractions run on mma.sync m16n8k16 with ldmatrix fragments (consume_f16, pd_k1_pipe.cuh): the weight rows are the
 // MMA's M side (16-row tiles), the batch rows its N side, accumulators in registers.
 //
+// Stacked GRU (layers = L, 2..4; rnn.py:40-67): phase B runs once per layer, with a grid barrier after each, so a step has
+// L - 1 more dependent phases.  Layer 0 contracts za with its W_ih; layer l > 0 the fp16 h' that layer l - 1 just wrote to
+// h16 (its D/L columns, a strided TMA map) with its own W_ih.  Phase C is unchanged: it contracts h' with the block-diagonal
+// [3D, D] W_hh the host assembles (each unit's row holds its layer's weights in its layer's columns and zeros elsewhere), so
+// every unit's partial sums cover only its own layer.  The previous h of a unit comes from hin (global) instead of the
+// shared-memory copy the single cell keeps.
+//
 // Batch rows beyond one 64-row MMA operand (IWAE: BI = B x iwae_samples, world.py:60-68 repeats every sequence I times) run in
 // the MULTI instantiation: phases B and C repeat their contraction and epilogue per block of 64 rows, phase D takes 64 rows
 // per pass with all eight warps, and the row owners of A / C' stride over the rows by the grid size.
@@ -52,6 +59,8 @@ struct FwdMaps {
     CUtensorMap wih3;                          // W_ih as (k, unit, gate): box {64 halfs, 16 units, 3 gates} = tiles 0..2 of phase B
     CUtensorMap whh3;                          // W_hh as (k, unit, gate): box {64 halfs, 64 units, 3 gates} = tiles 0..11 of phase C
     CUtensorMap wph32, wpm32;                  // box {64 halfs, 32 rows} = tiles 12, 13 of phase C / the two class tiles of phase D
+    CUtensorMap hl[3];                         // stacked GRU: h16 columns of layer l - 1 ([BI, D/L] at ld D), input of layer l's phase B
+    CUtensorMap wih3l[3];                      // stacked GRU: W_ih of layer l as (k, unit, gate), box {64 halfs, 16 units, 3 gates}
 };
 
 // LayerNorm + ELU of one row held as v[4] per consumer thread (features tid + 256 i); writes fp32 (fp16-representable) and
@@ -101,6 +110,7 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     const int P = gridDim.x, c = blockIdx.x;
     const int T = a.T, BI = a.BI, D = a.D, Hd = a.Hd, G = a.G, C = a.C, Z = G * C, F = D + Z, D3 = 3 * D;
     const int Bq = BI / a.I;                                // sequences (rows of aa / ea per timestep)
+    const int L = a.layers > 1 ? a.layers : 1, Dl = D / L;  // GRU layers, units per layer
     const __half* wzT = (const __half*)a.ws_wzT16;          // [Z][Hd], transposed z_mlp weight (written by the host)
     __half* za16 = (__half*)a.ws_za16;
     __half* h16 = (__half*)a.ws_h16;
@@ -110,7 +120,8 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
     ring.init(smem, (uint64_t*)(smem + OFF_BAR));
 
     // ---- static ownership
-    const int u4_0 = (int)((long)c * D / P), u4_1 = (int)((long)(c + 1) * D / P), nu = u4_1 - u4_0;   // B: my hidden units
+    // B: my hidden units of layer l are [l Dl + u4_0, l Dl + u4_1)
+    const int u4_0 = (int)((long)c * Dl / P), u4_1 = (int)((long)(c + 1) * Dl / P), nu = u4_1 - u4_0;
     const int RG = P / KS, rg = c / KS, ks = c % KS;                                                    // C: row group x k slice
     const bool inC = rg < RG;
     const int u6_0 = (int)((long)rg * D / RG), u6_1 = inC ? (int)((long)(rg + 1) * D / RG) : u6_0;     // C: gh rows (units)
@@ -129,10 +140,11 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
 
     // weight tiles come in grouped boxes (FwdMaps); phase D takes one box per 16-row tile unless its C classes fill two tiles.
     // Jobs B and C always set ngop > 0 and leave wmap / row0 unset: produce() does not read them then.
-    auto job_b = [&]() {
-        JobF j; j.ntile = nu > 0 ? 3 : 0; j.nx = 1; j.xmap[0] = &maps.za; j.xmap[1] = &maps.za; j.xrow0 = 0; j.xrows = BROWS; j.xf16 = 1;
-        j.kcol0 = 0; j.nkb = j.ntile ? (Hd + KB - 1) / KB : 0; j.x2_from = 1 << 30;
-        j.ngop = 1; j.gmap[0] = &maps.wih3; j.grow[0] = u4_0; j.gdst[0] = 0; j.g3d[0] = 1;
+    auto job_b = [&](int l) {                                       // phase B of GRU layer l
+        const CUtensorMap* xm = l == 0 ? &maps.za : &maps.hl[l - 1];
+        JobF j; j.ntile = nu > 0 ? 3 : 0; j.nx = 1; j.xmap[0] = xm; j.xmap[1] = xm; j.xrow0 = 0; j.xrows = BROWS; j.xf16 = 1;
+        j.kcol0 = 0; j.nkb = j.ntile ? ((l == 0 ? Hd : Dl) + KB - 1) / KB : 0; j.x2_from = 1 << 30;
+        j.ngop = 1; j.gmap[0] = l == 0 ? &maps.wih3 : &maps.wih3l[l - 1]; j.grow[0] = u4_0; j.gdst[0] = 0; j.g3d[0] = 1;
         return j;
     };
     auto job_c = [&]() {
@@ -161,11 +173,15 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             { const JobF j = job_c(); if (j.nkb) for (int bb = 0; bb < NBB; ++bb) produce(ring, j, a.ws_barrier, 1, bb * BROWS); }
             epoch = 2;
             for (int t = 0; t < T; ++t) {
-                // barriers of a step: after A (1), after B (2), after C (3), after C' (4), after D (5, not on the last step)
-                { const JobF j = job_b(); if (j.nkb) for (int bb = 0; bb < NBB; ++bb) produce(ring, j, a.ws_barrier, epoch + 1, bb * BROWS); }
-                { const JobF j = job_c(); if (j.nkb) for (int bb = 0; bb < NBB; ++bb) produce(ring, j, a.ws_barrier, epoch + 2, bb * BROWS); }
-                { const JobF j = job_d(); if (j.nkb) for (int rc = 0; rc < NDC; ++rc) produce(ring, j, a.ws_barrier, epoch + 4, rc * DR); }
-                epoch += 5;
+                // barriers of a step: after A (1), after B of layer l (2 + l), after C (2 + L), after C' (3 + L), after D
+                // (4 + L, not on the last step)
+                for (int l = 0; l < L; ++l) {
+                    const JobF j = job_b(l);
+                    if (j.nkb) for (int bb = 0; bb < NBB; ++bb) produce(ring, j, a.ws_barrier, epoch + 1 + l, bb * BROWS);
+                }
+                { const JobF j = job_c(); if (j.nkb) for (int bb = 0; bb < NBB; ++bb) produce(ring, j, a.ws_barrier, epoch + 1 + L, bb * BROWS); }
+                { const JobF j = job_d(); if (j.nkb) for (int rc = 0; rc < NDC; ++rc) produce(ring, j, a.ws_barrier, epoch + 3 + L, rc * DR); }
+                epoch += 4 + L;
             }
         }
         return;
@@ -277,9 +293,13 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
         }
         grid_barrier(a.ws_barrier, epoch);                                      // (1) za complete
 
-        // ---- phase B (hidden-unit owners): gi = za . W_ih^T, GRU gate math, h' -> feat / hin[t+1] / h16
-        {
-            const JobF j = job_b();
+        // ---- phase B (hidden-unit owners), once per GRU layer: gi = x . W_ih^T (x = za, or layer l - 1's h'), GRU gate math,
+        //      h' -> feat / hin[t+1] / h16
+        for (int l = 0; l < L; ++l) {
+            const JobF j = job_b(l);
+            const int uoff = l * Dl;                                    // first unit of the layer
+            const float* b_ih = l == 0 ? a.b_ih : a.b_ih_l[l - 1];
+            const float* b_hh = l == 0 ? a.b_hh : a.b_hh_l[l - 1];
             if (j.nkb > 0) {
               for (int bb = 0; bb < NBB; ++bb) {
                 if (MULTI && bb > 0) cons_sync();                          // gis of the previous block has been read
@@ -309,7 +329,7 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
                         const int o = o0 + q * NCT;
                         gh[q][0] = gh[q][1] = gh[q][2] = 0.f;
                         if (o < nu * nb) {
-                            const int u = u4_0 + o % nu, b = bb * BROWS + o / nu;
+                            const int u = uoff + u4_0 + o % nu, b = bb * BROWS + o / nu;
                             for (int k = 0; k < KS; ++k) {                  // threads run over u: coalesced
                                 const float* gp = a.ws_ghpart + ((long)k * BI + b) * D3 + u;
                                 gh[q][0] += __ldcg(gp); gh[q][1] += __ldcg(gp + D); gh[q][2] += __ldcg(gp + 2 * D);
@@ -320,35 +340,35 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
                     for (int q = 0; q < 4; ++q) {
                         const int o = o0 + q * NCT;
                         if (o >= nu * nb) break;
-                        const int r = o % nu, bl = o / nu, b = bb * BROWS + bl, u = u4_0 + r;
+                        const int r = o % nu, bl = o / nu, b = bb * BROWS + bl, ul = u4_0 + r, u = uoff + ul;
                         const long row = (long)t * BI + b;
                         const float m = t > 0 ? a.mask[row] : 1.f;              // h_0 arrives already masked
                         const float mn = t + 1 < T ? a.mask[row + BI] : 0.f;
-                        const float ghr = m * gh[q][0] + a.b_hh[u];
-                        const float ghu = m * gh[q][1] + a.b_hh[D + u];
-                        const float ghn = m * gh[q][2] + a.b_hh[2 * D + u];
-                        const float rg_ = pd_sigmoid(gis[(0 * 16 + r) * 65 + bl] + a.b_ih[u] + ghr);
-                        const float ug_ = pd_sigmoid(gis[(1 * 16 + r) * 65 + bl] + a.b_ih[D + u] + ghu);
-                        const float ng_ = tanhf(gis[(2 * 16 + r) * 65 + bl] + a.b_ih[2 * D + u] + rg_ * ghn);
-                        const float hp = hcs[r * HS + b];
+                        const float ghr = m * gh[q][0] + b_hh[ul];
+                        const float ghu = m * gh[q][1] + b_hh[Dl + ul];
+                        const float ghn = m * gh[q][2] + b_hh[2 * Dl + ul];
+                        const float rg_ = pd_sigmoid(gis[(0 * 16 + r) * 65 + bl] + b_ih[ul] + ghr);
+                        const float ug_ = pd_sigmoid(gis[(1 * 16 + r) * 65 + bl] + b_ih[Dl + ul] + ghu);
+                        const float ng_ = tanhf(gis[(2 * 16 + r) * 65 + bl] + b_ih[2 * Dl + ul] + rg_ * ghn);
+                        const float hp = L == 1 ? hcs[r * HS + b] : __ldcg(a.hin + row * D + u);
                         const __half hh = __float2half_rn((1.f - ug_) * ng_ + ug_ * hp);
                         const float hn = __half2float(hh);
                         a.feat[row * F + u] = hn;
                         h16[(long)b * D + u] = hh;
                         hcs[r * HS + b] = hn * mn;
                         if (t + 1 < T) a.hin[(row + BI) * D + u] = hn * mn;
-                        float* gt = a.gates + row * 4 * D;
-                        gt[u] = rg_; gt[D + u] = ug_; gt[2 * D + u] = ng_; gt[3 * D + u] = ghn;
+                        float* gt = a.gates + (((long)l * T + t) * BI + b) * 4 * Dl;        // [L, T, BI, 4 Dl]
+                        gt[ul] = rg_; gt[Dl + ul] = ug_; gt[2 * Dl + ul] = ng_; gt[3 * Dl + ul] = ghn;
                     }
                 }
               }
             }
+            grid_barrier(a.ws_barrier, epoch);                                  // (2 + l) h' of layer l complete
         }
-        grid_barrier(a.ws_barrier, epoch);                                      // (2) h' complete
 
         // ---- phase C: partials of y2 = h' . W_ph^T and of gh_{t+1} = h' . W_hh^T
         phase_c(t + 1 < T, true);
-        grid_barrier(a.ws_barrier, epoch);                                      // (3) partials complete
+        grid_barrier(a.ws_barrier, epoch);                                      // (2 + L) partials complete
 
         // ---- phase C' (CTA b < BI): y2 = partial sums + b_ph + ea_t ; LayerNorm + ELU -> pin
         for (int b = c; b < BI; b += ASTEP) {
@@ -367,7 +387,7 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
             }
             ln_elu_row(v, Hd, a.ln2_g, a.ln2_b, a.eps, a.pin + row * Hd, pin16 + (long)b * Hd, a.m2 + row, a.r2 + row, sh);
         }
-        grid_barrier(a.ws_barrier, epoch);                                      // (4) pin complete
+        grid_barrier(a.ws_barrier, epoch);                                      // (3 + L) pin complete
 
         // ---- phase D (latent-group owners): logits of group g for my rows, softmax, argmax(p / q) -> post, idx, z
         for (int rc = 0; rc < NDC; ++rc) {
@@ -420,7 +440,7 @@ __global__ void __launch_bounds__(NT, 1) rssm_unroll_fwd3_kernel(const pd_rssm_f
                 if (lane == 0) a.idx[row * G + g9] = k;
             }
         }
-        if (t + 1 < T) grid_barrier(a.ws_barrier, epoch);                       // (5) idx_t complete
+        if (t + 1 < T) grid_barrier(a.ws_barrier, epoch);                       // (4 + L) idx_t complete
     }
 }
 
@@ -444,6 +464,10 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     const int P = h->k1_ctas;
     PD_REQUIRE(h, P > 0, "pd_rssm_unroll_fwd: kernel does not fit an SM");
     const int Z = a->G * a->C;
+    const int L = a->layers > 1 ? a->layers : 1;
+    const int Dl = a->D / L;
+    bool layers_ok = a->layers >= 0 && a->layers <= 4 && a->D % L == 0 && Dl % 8 == 0;
+    for (int l = 1; l < L; ++l) layers_ok = layers_ok && a->w_ih16_l[l - 1] && a->b_ih_l[l - 1] && a->b_hh_l[l - 1];
     const int KS = (a->D % (KSPLIT * KB) == 0 && P >= KSPLIT) ? KSPLIT : 1;
     const int RG = P / KS;
     const int R = P / a->G < 4 ? (P / a->G < 1 ? 1 : P / a->G) : 4;
@@ -451,11 +475,11 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     const bool multi = !(a->BI <= BROWS && a->BI <= P && (a->BI + R - 1) / R <= 16);
     const bool ok = a->T >= 1 && a->BI >= 1 && a->BI <= HB && a->I >= 1 && a->BI % a->I == 0 &&
                     a->Hd <= 4 * NCT && a->Hd % 8 == 0 && a->D % 8 == 0 && a->C >= 1 && a->C <= 32 && a->G >= 1 && a->G <= P && a->G <= MAXG &&
-                    (a->D + P - 1) / P <= 16 && (a->D + RG - 1) / RG <= 64 &&
+                    layers_ok && (Dl + P - 1) / P <= 16 && (a->D + RG - 1) / RG <= 64 &&
                     (a->Hd + RG - 1) / RG <= 32 && Z >= 1 && a->ws_ghpart && a->ws_y2part && a->ws_wzT16;
     if (!ok)
-        PD_FAIL(h, PD_ERR_UNSUPPORTED, "pd_rssm_unroll_fwd: shape T=%d BI=%d D=%d Hd=%d G=%d C=%d outside the kernel's limits",
-                a->T, a->BI, a->D, a->Hd, a->G, a->C);
+        PD_FAIL(h, PD_ERR_UNSUPPORTED, "pd_rssm_unroll_fwd: shape T=%d BI=%d D=%d Hd=%d G=%d C=%d layers=%d outside the kernel's limits",
+                a->T, a->BI, a->D, a->Hd, a->G, a->C, a->layers);
     FwdMaps maps;
     memset(&maps, 0, sizeof(maps));
     const char* who = "pd_rssm_unroll_fwd";
@@ -464,7 +488,11 @@ extern "C" int pd_rssm_unroll_fwd(pd_handle* h, const pd_rssm_fwd_args* a, void*
     if (!rc) rc = make_map(h, who, &maps.h, a->ws_h16, a->BI, a->D, BROWS, true);
     if (!rc) rc = make_map(h, who, &maps.pin16, a->ws_pin16, a->BI, a->Hd, 16, true);
     if (!rc) rc = make_map(h, who, &maps.pin64, a->ws_pin16, a->BI, a->Hd, BROWS, true);
-    if (!rc) rc = make_map3g(h, who, &maps.wih3, a->w_ih16, a->D, a->Hd, 3, 16);
+    if (!rc) rc = make_map3g(h, who, &maps.wih3, a->w_ih16, Dl, a->Hd, 3, 16);
+    for (int l = 1; l < L && !rc; ++l) {
+        rc = make_map(h, who, &maps.hl[l - 1], (const __half*)a->ws_h16 + (long)(l - 1) * Dl, a->BI, Dl, BROWS, true, a->D);
+        if (!rc) rc = make_map3g(h, who, &maps.wih3l[l - 1], a->w_ih16_l[l - 1], Dl, Dl, 3, 16);
+    }
     if (!rc) rc = make_map3g(h, who, &maps.whh3, a->w_hh16, a->D, a->D, 3, 64);
     if (!rc) rc = make_map(h, who, &maps.wph32, a->w_ph16, a->Hd, a->D, 32, true);
     if (!rc) rc = make_map(h, who, &maps.wpm32, a->w_pm16, Z, a->Hd, 32, true);

@@ -252,21 +252,29 @@ class _MultiDecoder(nn.Module):
 
 
 class _GRUStack(nn.Module):
-    def __init__(self, input_size, hidden_size):
+    """rnn.py:40-67 (GRUCellStack, cell_type gru): num_layers cells of hidden_size / num_layers units.  Layer 0 reads the
+    input, layer l > 0 the new state of layer l - 1; the state is the concatenation of the layers' states."""
+
+    def __init__(self, input_size, hidden_size, num_layers):
         super().__init__()
-        self.layers = nn.ModuleList([nn.GRUCell(input_size, hidden_size)])
+        self.num_layers = num_layers
+        layer_size = hidden_size // num_layers
+        if layer_size * num_layers != hidden_size:
+            raise AssertionError("Must be divisible")                                        # rnn.py:45
+        self.layers = nn.ModuleList([nn.GRUCell(input_size, layer_size)] +
+                                    [nn.GRUCell(layer_size, layer_size) for _ in range(num_layers - 1)])
 
 
 class _RSSMCell(nn.Module):
     """rssm.py:96-116"""
 
-    def __init__(self, embed_dim, action_dim, deter_dim, stoch_dim, stoch_discrete, hidden_dim):
+    def __init__(self, embed_dim, action_dim, deter_dim, stoch_dim, stoch_discrete, hidden_dim, gru_layers):
         super().__init__()
         z = stoch_dim * stoch_discrete
         self.z_mlp = nn.Linear(z, hidden_dim)
         self.a_mlp = nn.Linear(action_dim, hidden_dim, bias=False)
         self.in_norm = nn.LayerNorm(hidden_dim, eps=1e-3)
-        self.gru = _GRUStack(hidden_dim, deter_dim)
+        self.gru = _GRUStack(hidden_dim, deter_dim, gru_layers)
         self.prior_mlp_h = nn.Linear(deter_dim, hidden_dim)
         self.prior_norm = nn.LayerNorm(hidden_dim, eps=1e-3)
         self.prior_mlp = nn.Linear(hidden_dim, z)
@@ -302,15 +310,15 @@ class _WorldModel(nn.Module):
         super().__init__()
         if not conf.stoch_discrete:
             raise NotImplementedError("Gaussian latents (stoch_discrete=0) are outside the accelerated path (§8f N4)")
-        if conf.gru_layers != 1 or conf.gru_type != "gru":
-            raise NotImplementedError("accelerated path covers gru_type=gru, gru_layers=1 (SURVEY.md §2 row 3)")
+        if conf.gru_type != "gru" or conf.gru_layers < 1:
+            raise NotImplementedError("accelerated path covers gru_type=gru with gru_layers >= 1 (SURVEY.md §2 row 3)")
         if conf.stoch_discrete > 32 or conf.stoch_dim > 32:
             raise NotImplementedError("categorical kernels handle <= 32 groups of <= 32 classes")
         self.encoder = _MultiEncoder(conf)
         features_dim = conf.deter_dim + conf.stoch_dim * conf.stoch_discrete
         self.decoder = _MultiDecoder(features_dim, conf)
         self.core = _RSSMCore(self.encoder.out_dim, conf.action_dim, conf.deter_dim, conf.stoch_dim,
-                              conf.stoch_discrete, conf.hidden_dim)
+                              conf.stoch_discrete, conf.hidden_dim, conf.gru_layers)
         # dreamer.py:267-279: the auxiliary critic learns the value of the observed rewards on the posterior features; its
         # actor is built (state_dict keys) but never trained
         self.ac_aux = _ActorCritic(features_dim, conf.action_dim, conf.layer_norm, conf.actor_dist) if conf.aux_critic else None
@@ -504,7 +512,8 @@ class Dreamer(nn.Module):
         self._catreward = isinstance(rew, _SupportHead)
         S = rew._support.numel() if self._catreward else 1
         # embedding = cat(image part [Ei], vecobs part [Ev]); each part has its own buffer and meets W_pe's column slice
-        self.d = SimpleNamespace(D=conf.deter_dim, G=conf.stoch_dim, C=conf.stoch_discrete,
+        self.d = SimpleNamespace(D=conf.deter_dim, L=conf.gru_layers, Dl=conf.deter_dim // conf.gru_layers,  # Dl: units per GRU layer
+                                 G=conf.stoch_dim, C=conf.stoch_discrete,
                                  Z=conf.stoch_dim * conf.stoch_discrete, Hd=conf.hidden_dim, E=enc.out_dim,
                                  Ei=enc.encoder_image.out_dim if enc.encoder_image is not None else 0,
                                  Ev=enc.encoder_vecobs.out_dim if enc.encoder_vecobs is not None else 0,
@@ -770,7 +779,17 @@ class Dreamer(nn.Module):
             wz = self.wm.core.cell.z_mlp.weight
             self._k1_wzT = self._buf("k1.wzT", wz.shape[1], wz.shape[0], dtype=torch.float16)
             ops.transpose_to_half(self._raw(wz), self._k1_wzT)
-        if self.persistent_bptt:      # transposed fp16 copies: operands of the persistent BPTT kernel (pd_rssm_unroll_bwd)
+            d = self.d
+            if d.L > 1 and self._fp16_forward_ok():
+                # a stacked GRU's recurrent weights as the block-diagonal [3D, D] fp16 matrix the persistent unroll contracts
+                # (row gate * D + u: unit u's row of its layer's W_hh in that layer's columns; the zeros are never written)
+                self._k1_whh = self._buf("k1.whh_bd", 3 * d.D, d.D, dtype=torch.float16, zero=True)
+                for l, g_ in enumerate(self.wm.core.cell.gru.layers):
+                    cl = self._gru_cols(l)
+                    for gate in range(3):
+                        ops.to_half(self._raw(g_.weight_hh)[gate * d.Dl:(gate + 1) * d.Dl],
+                                    self._k1_whh[gate * d.D + l * d.Dl:gate * d.D + (l + 1) * d.Dl, cl])
+        if self.persistent_bptt and self.d.L == 1:     # transposed fp16 copies: operands of pd_rssm_unroll_bwd (one cell)
             cell = self.wm.core.cell
             gru = cell.gru.layers[0]
             self._k1b_w = {}
@@ -1035,7 +1054,7 @@ class Dreamer(nn.Module):
 
     def _persistent_bptt_ok(self, BI):
         d, P = self.d, _persistent_sms(self, self.persistent_bptt and getattr(self, "_k1b_w", None))
-        if P is None:
+        if P is None or getattr(d, "L", 1) > 1:         # the kernel contracts one GRU cell (d without L: one cell)
             return False
         Z = d.G * d.C
         ks2 = 4 if Z % 256 == 0 and P >= 4 else 1
@@ -1053,13 +1072,17 @@ class Dreamer(nn.Module):
             return False
         ks = 4 if d.D % 256 == 0 and P >= 4 else 1
         cd = lambda a_, b_: -(-a_ // b_)
+        # a stacked GRU: up to 4 layers of Dl = D / L units, Dl a multiple of 8 (the fp16 TMA maps of its column slices);
+        # phase B spreads one layer's units over the P CTAs (d without L: one cell)
+        L, Dl = getattr(d, "L", 1), getattr(d, "Dl", d.D)
         # batch rows (B x iwae_samples) beyond one 64-row MMA operand are taken in blocks by the kernel, up to 256; at most
         # 256 latent groups (MAXG of csrc/pd_rssm_fwd3.cu)
         return (BI <= 256 and d.Hd <= 1024 and d.Hd % 8 == 0 and d.D % 8 == 0 and d.C <= 32 and d.G <= min(P, 256) and
-                cd(d.D, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32)
+                L <= 4 and Dl % 8 == 0 and cd(Dl, P) <= 16 and cd(d.D, P // ks) <= 64 and cd(d.Hd, P // ks) <= 32)
 
     def _fp16_forward_ok(self):
-        return _fp16_path_ok(self)
+        # a stacked GRU's layers read and write column slices of D / L units: D / L too must be a multiple of 8 halves
+        return _fp16_path_ok(self) and self.d.Dl % 8 == 0
 
     def _implicit_conv_ok(self):
         """The implicit-GEMM convolutions (pd_conv_gemm) run when switched on and every activation they read or write has
@@ -1126,6 +1149,10 @@ class Dreamer(nn.Module):
         return dict(wm_out, out_state=tuple(s_.clone() for s_ in wm_out["out_state"])), ac_out
 
     # ------------------------------------------------------------------ world model forward
+    def _gru_cols(self, l):
+        """The units of GRU layer l in a D-wide state row (rnn.py:63, state.chunk(num_layers, -1))."""
+        return slice(l * self.d.Dl, (l + 1) * self.d.Dl)
+
     def _rssm_head(self, prior):
         """(Linear, LayerNorm, Linear) computing the prior logits (from h) or the posterior ones (from h and the embedding)."""
         c = self.wm.core.cell
@@ -1138,7 +1165,7 @@ class Dreamer(nn.Module):
         NB, BI = T * B, B * I
         b = lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)
         cell = self.wm.core.cell
-        gru = cell.gru.layers[0]
+        gru = cell.gru.layers[0]                # layer 0 (the only one of a single cell)
         ea = b("rssm.ea", NB, d.Hd)
         w_pe = self._w(cell.post_mlp_e.weight)         # [Hd, E]: columns [0, Ei) meet the image part, [Ei, E) the vecobs part
         img = embed = enc_in = denc = None
@@ -1217,9 +1244,13 @@ class Dreamer(nn.Module):
                 Wh, h16 = self._wh, torch.float16
                 ops.gemm(zin[0], W(cell.z_mlp.weight), x1[0], bias=self._raw(cell.z_mlp.bias), res=aa[:B], r_div=I)
                 ph, pn, pm = head
+                grus = cell.gru.layers
                 ops.rssm_unroll_fwd(
-                    dict(T=T, BI=BI, I=I, D=d.D, Hd=d.Hd, G=d.G, C=d.C), 1e-3,
-                    w_z16=Wh(cell.z_mlp.weight), w_ih16=Wh(gru.weight_ih), w_hh16=Wh(gru.weight_hh), w_ph16=Wh(ph.weight),
+                    dict(T=T, BI=BI, I=I, D=d.D, Hd=d.Hd, G=d.G, C=d.C, layers=d.L if d.L > 1 else 0), 1e-3,
+                    w_z16=Wh(cell.z_mlp.weight), w_ih16=Wh(gru.weight_ih),
+                    w_hh16=Wh(gru.weight_hh) if d.L == 1 else self._k1_whh, w_ph16=Wh(ph.weight),
+                    w_ih16_l=[Wh(g_.weight_ih) for g_ in grus[1:]], b_ih_l=[self._raw(g_.bias_ih) for g_ in grus[1:]],
+                    b_hh_l=[self._raw(g_.bias_hh) for g_ in grus[1:]],
                     w_pm16=Wh(pm.weight), b_z=self._raw(cell.z_mlp.bias), ln1_g=self._raw(cell.in_norm.weight),
                     ln1_b=self._raw(cell.in_norm.bias), b_ih=self._raw(gru.bias_ih), b_hh=self._raw(gru.bias_hh),
                     b_ph=self._raw(ph.bias), ln2_g=self._raw(pn.weight), ln2_b=self._raw(pn.bias), b_pm=self._raw(pm.bias),
@@ -1241,25 +1272,33 @@ class Dreamer(nn.Module):
             for buf_ in (x1, gi, gh, y2, post):
                 ops.fill(buf_, 0.0)
         par = self._ov(2)
-        gh_gemm = lambda t: ops.gemm(hin[t], W(gru.weight_hh), gh[t], bias=self._raw(gru.bias_hh), c_zeroed=skinny)
+        # GRU layer l (rnn.py:60-67) owns the units col(l) of the state rows; its gates / products are rows [l, t] of the
+        # (L, T, BI, ·) views (the (T, BI, ·) buffers themselves when L = 1)
+        grus, col = cell.gru.layers, self._gru_cols
+        gil, ghl, gatesl = (x.view(d.L, T, BI, -1) for x in (gi, gh, gates))
+        gh_gemm = lambda t, l: ops.gemm(hin[t][:, col(l)], W(grus[l].weight_hh), ghl[l, t], bias=self._raw(grus[l].bias_hh),
+                                        c_zeroed=skinny)
         if par:
             with self._fork(2):
-                gh_gemm(0)
+                for l in range(d.L):
+                    gh_gemm(0, l)
         for t in range(T):
             last = t == T - 1
             ops.gemm(zin[t], W(cell.z_mlp.weight), x1[t], bias=self._raw(cell.z_mlp.bias), res=aa[t * B:(t + 1) * B],
                      r_div=I, c_zeroed=skinny)
             ops.ln_elu_fwd(x1[t], self._raw(cell.in_norm.weight), self._raw(cell.in_norm.bias), 1e-3, za[t], m1[t], r1[t])
-            ops.gemm(za[t], W(gru.weight_ih), gi[t], bias=self._raw(gru.bias_ih), c_zeroed=skinny)
-            if par:
-                self._join(2)
-            else:
-                gh_gemm(t)
-            ops.gru_fwd(gi[t], gh[t], hin[t], feat[t, :, :d.D], None if last else hin[t + 1],
-                        None if last else mask[t + 1], gates[t])
-            if par and not last:                    # h_{t+1} is known: its W_hh product overlaps the posterior MLP
-                with self._fork(2):
-                    gh_gemm(t + 1)
+            for l in range(d.L):                    # layer l > 0 reads layer l - 1's new state
+                ops.gemm(za[t] if l == 0 else feat[t, :, col(l - 1)], W(grus[l].weight_ih), gil[l, t],
+                         bias=self._raw(grus[l].bias_ih), c_zeroed=skinny)
+                if not par:
+                    gh_gemm(t, l)
+                elif l == 0:
+                    self._join(2)
+                ops.gru_fwd(gil[l, t], ghl[l, t], hin[t][:, col(l)], feat[t, :, col(l)],
+                            None if last else hin[t + 1][:, col(l)], None if last else mask[t + 1], gatesl[l, t])
+                if par and not last:                # h_{t+1} of this layer is known: its W_hh product overlaps what follows
+                    with self._fork(2):
+                        gh_gemm(t + 1, l)
             self._head_fwd(head, feat[t, :, :d.D], y2[t], pin[t], m2[t], r2[t], post[t],
                            res=None if open_loop else ea[t * B:(t + 1) * B], r_div=1 if open_loop else I, c_zeroed=skinny)
             ops.cat_sample(post[t], noise_post[t], d.G, d.C, feat[t, :, d.D:], None if last else zin[t + 1],
@@ -1483,7 +1522,6 @@ class Dreamer(nn.Module):
         N = NB * I
         b, W, G = self._buf, self._w, self._g
         cell = self.wm.core.cell
-        gru = cell.gru.layers[0]
         featN, w, dd = fw.featN, fw.w, fw.dec
         dfeat = b("bwd.dfeat", N, d.F)
         par_w = self._conv and self._ov(4)      # image weight gradients leave the dfeat -> BPTT critical path (joined at the end)
@@ -1531,6 +1569,8 @@ class Dreamer(nn.Module):
         dpin, dza = b("bwd.dpin", T, BI, d.Hd), b("bwd.dza", T, BI, d.Hd)
         dhp, dhc = b("bwd.dhp", T, BI, d.D), b("bwd.dhc", BI, d.D)
         dhin, dzin = b("bwd.dhin", T, BI, d.D), b("bwd.dzin", T, BI, d.Z)
+        grus, col = cell.gru.layers, self._gru_cols
+        gatesl, dgil, dghl = (x.view(d.L, T, BI, -1) for x in (gates, dgi, dgh))
         done = False
         if self._persistent_bptt_ok(BI):
             try:
@@ -1558,11 +1598,17 @@ class Dreamer(nn.Module):
             ops.gemm(dy2[t], W(cell.post_mlp_h.weight), dhp[t], b_mn=True, res=dfeat3[t, :, :d.D])
             if par and nxt:
                 self._join(2)                       # dhin[t + 1]
-            ops.gru_bwd(dhp[t], dhin[t + 1] if nxt else None, mask[t + 1] if nxt else None, gates[t], hin[t], dgi[t],
-                        dgh[t], dhc)
-            with self._fork(2) if par else contextlib.nullcontext():
-                ops.gemm(dgh[t], W(gru.weight_hh), dhin[t], b_mn=True, res=dhc)
-            ops.gemm(dgi[t], W(gru.weight_ih), dza[t], b_mn=True)
+            for l in reversed(range(d.L)):          # layer l's input gradient joins layer l - 1's output gradient
+                c = col(l)
+                ops.gru_bwd(dhp[t][:, c], dhin[t + 1][:, c] if nxt else None, mask[t + 1] if nxt else None, gatesl[l, t],
+                            hin[t][:, c], dgil[l, t], dghl[l, t], dhc[:, c])
+                with self._fork(2) if par else contextlib.nullcontext():
+                    ops.gemm(dghl[l, t], W(grus[l].weight_hh), dhin[t][:, c], b_mn=True, res=dhc[:, c])
+                if l > 0:
+                    dx = dhp[t][:, col(l - 1)]
+                    ops.gemm(dgil[l, t], W(grus[l].weight_ih), dx, b_mn=True, res=dx)
+                else:
+                    ops.gemm(dgil[0, t], W(grus[0].weight_ih), dza[t], b_mn=True)
             ops.ln_elu_bwd(dza[t], x1[t], za[t], self._raw(cell.in_norm.weight), m1[t], r1[t], dx1[t],
                            G(cell.in_norm.weight), G(cell.in_norm.bias), G(cell.z_mlp.bias))
             ops.gemm(dx1[t], W(cell.z_mlp.weight), dzin[t], b_mn=True)
@@ -1573,10 +1619,12 @@ class Dreamer(nn.Module):
         ops.gemm(f2(dpost), f2(pin), G(cell.post_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
         ops.colsum(f2(dpost), G(cell.post_mlp.bias))
         ops.gemm(f2(dy2), featN[:, :d.D], G(cell.post_mlp_h.weight), a_mn=True, b_mn=True, accumulate=True)
-        ops.gemm(f2(dgh), f2(hin), G(gru.weight_hh), a_mn=True, b_mn=True, accumulate=True)
-        ops.colsum(f2(dgh), G(gru.bias_hh))
-        ops.gemm(f2(dgi), f2(za), G(gru.weight_ih), a_mn=True, b_mn=True, accumulate=True)
-        ops.colsum(f2(dgi), G(gru.bias_ih))
+        for l, g_ in enumerate(grus):               # layer l's rows of dgi / dgh, its column slices of hin / h'
+            ops.gemm(dghl[l].reshape(N, -1), f2(hin)[:, col(l)], G(g_.weight_hh), a_mn=True, b_mn=True, accumulate=True)
+            ops.colsum(dghl[l].reshape(N, -1), G(g_.bias_hh))
+            ops.gemm(dgil[l].reshape(N, -1), f2(za) if l == 0 else featN[:, col(l - 1)], G(g_.weight_ih), a_mn=True,
+                     b_mn=True, accumulate=True)
+            ops.colsum(dgil[l].reshape(N, -1), G(g_.bias_ih))
         ops.gemm(f2(dx1), f2(zin), G(cell.z_mlp.weight), a_mn=True, b_mn=True, accumulate=True)
         if I == 1:
             dea, daa = f2(dy2), f2(dx1)
@@ -1714,7 +1762,7 @@ class Dreamer(nn.Module):
         ops, d, conf = self.ops, self.d, self.conf
         b, W = (lambda name, *shape, **kw: self._buf(tag + name, *shape, **kw)), self._w
         cell = self.wm.core.cell
-        gru = cell.gru.layers[0]
+        grus, col = cell.gru.layers, self._gru_cols
         ap = self._mlp_params(self.ac.actor)
         f16 = self._fp16_forward_ok()
         dr = SimpleNamespace(alog=b("dream.alog", H, N, d.Ap)[..., :d.Aout], actions=b("dream.actions", H, N, d.A),
@@ -1723,7 +1771,7 @@ class Dreamer(nn.Module):
         aidx = b("dream.aidx", N, 1, dtype=torch.int32)
         aa, x, za = b("dream.aa", N, d.Hd), b("dream.x", N, d.Hd), b("dream.za", N, d.Hd)
         mm, rr = b("dream.m", N), b("dream.r", N)
-        gi, gh = b("dream.gi", N, 3 * d.D), b("dream.gh", N, 3 * d.D)
+        gi, gh = (b(n_, N, 3 * d.D).view(d.L, N, 3 * d.Dl) for n_ in ("dream.gi", "dream.gh"))     # [l]: GRU layer l
         yp, pp, prior = b("dream.yp", N, d.Hd), b("dream.pp", N, d.Hd), b("dream.prior", N, d.Z)
         za16, pp16 = (b("dream.za16", N, d.Hd, dtype=torch.float16), b("dream.pp16", N, d.Hd, dtype=torch.float16)) if f16 \
             else (None, None)
@@ -1731,10 +1779,11 @@ class Dreamer(nn.Module):
         if f16:
             ops.to_half(feats[0], fx[0])
         par = self._ov(2)
-        gh_gemm = lambda i: self._fgemm(fx[i][:, :d.D], gru.weight_hh, gh, f16, bias=self._raw(gru.bias_hh))
+        gh_gemm = lambda i, l: self._fgemm(fx[i][:, col(l)], grus[l].weight_hh, gh[l], f16, bias=self._raw(grus[l].bias_hh))
         if par:
             with self._fork(2):
-                gh_gemm(0)
+                for l in range(d.L):
+                    gh_gemm(0, l)
         for i in range(H):
             f, fn, xn = feats[i], feats[i + 1], fx[i + 1]
             self._mlp_fwd(ap, f, dr.alog[i], dr.actor, row0=i * N, x16=fx[i] if f16 else None)
@@ -1749,15 +1798,17 @@ class Dreamer(nn.Module):
                 ops.gemm(dr.actions[i], W(cell.a_mlp.weight), aa)
             self._fgemm(fx[i][:, d.D:], cell.z_mlp.weight, x, f16, bias=self._raw(cell.z_mlp.bias), res=aa)
             ops.ln_elu_fwd(x, self._raw(cell.in_norm.weight), self._raw(cell.in_norm.bias), 1e-3, za, mm, rr, za16)
-            self._fgemm(za16 if f16 else za, gru.weight_ih, gi, f16, bias=self._raw(gru.bias_ih))
-            if par:
-                self._join(2)
-            else:
-                gh_gemm(i)
-            ops.gru_fwd(gi, gh, f[:, :d.D], fn[:, :d.D], h16=xn[:, :d.D] if f16 else None)
-            if par and i + 1 < H:               # next step's h·W_hh overlaps prior MLP, sampling and the actor
-                with self._fork(2):
-                    gh_gemm(i + 1)
+            for l in range(d.L):                # layer l > 0 reads layer l - 1's new state (its fp16 copy on the fp16 path)
+                xl = (za16 if f16 else za) if l == 0 else (xn if f16 else fn)[:, col(l - 1)]
+                self._fgemm(xl, grus[l].weight_ih, gi[l], f16, bias=self._raw(grus[l].bias_ih))
+                if not par:
+                    gh_gemm(i, l)
+                elif l == 0:
+                    self._join(2)
+                ops.gru_fwd(gi[l], gh[l], f[:, col(l)], fn[:, col(l)], h16=xn[:, col(l)] if f16 else None)
+                if par and i + 1 < H:           # next step's h·W_hh overlaps prior MLP, sampling and the actor
+                    with self._fork(2):
+                        gh_gemm(i + 1, l)
             self._head_fwd(self._rssm_head(prior=True), xn[:, :d.D], yp, pp, mm, rr, prior, f16, pp16)
             ops.cat_sample(prior, noise_prior[i], d.G, d.C, fn[:, d.D:], z16=xn[:, d.D:] if f16 else None)
         return dr

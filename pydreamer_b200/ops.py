@@ -41,8 +41,10 @@ class RssmFwdArgs(ctypes.Structure):
               "ln2_g", "ln2_b", "b_pm")
     _PTRS2 = ("aa", "ea", "mask", "noise", "x1", "za", "m1", "r1", "gates", "feat", "hin", "zin", "y2", "pin", "m2",
               "r2", "post", "idx", "ws_wzT16", "ws_za16", "ws_h16", "ws_pin16", "ws_barrier", "ws_ghpart", "ws_y2part")
+    _LAYERS = ("w_ih16_l", "b_ih_l", "b_hh_l")                 # stacked GRU: layers 1 .. L-1
     _fields_ = ([(n, ctypes.c_int) for n in _INTS] + [(n, ctypes.c_void_p) for n in _PTRS1] +
-                [("eps", ctypes.c_float)] + [(n, ctypes.c_void_p) for n in _PTRS2])
+                [("eps", ctypes.c_float)] + [(n, ctypes.c_void_p) for n in _PTRS2] + [("layers", ctypes.c_int)] +
+                [(n, ctypes.c_void_p * 3) for n in _LAYERS])
 
 
 class RssmBwdArgs(ctypes.Structure):
@@ -184,12 +186,18 @@ class NativeOps:
                                      _ld(dh_carry), self._s()), "pd_gru_bwd")
 
     def rssm_unroll_fwd(self, dims, eps, **t):
-        """Persistent posterior unroll (pd_rssm_unroll_fwd).  dims = dict(T, BI, I, D, Hd, G, C); every other struct
-        field is passed as a contiguous tensor (or None) by its field name."""
+        """Persistent posterior unroll (pd_rssm_unroll_fwd).  dims = dict(T, BI, I, D, Hd, G, C, optional layers); every
+        other struct field is passed as a contiguous tensor (or None) by its field name, the per-layer ones (w_ih16_l,
+        b_ih_l, b_hh_l) as lists of the tensors of layers 1 .. L-1."""
         a = RssmFwdArgs()
         for n in RssmFwdArgs._INTS:
             setattr(a, n, int(dims[n]))
         a.eps = float(eps)
+        a.layers = int(dims.get("layers", 0))
+        for n in RssmFwdArgs._LAYERS:
+            for i, v in enumerate(t.pop(n, None) or ()):
+                assert v.is_contiguous(), n
+                getattr(a, n)[i] = v.data_ptr()
         for n in RssmFwdArgs._PTRS1 + RssmFwdArgs._PTRS2:
             v = t.pop(n, None)
             if v is not None:
