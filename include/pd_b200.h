@@ -379,6 +379,18 @@ int pd_actor_loss_tanh_normal(pd_handle* h, long rows, int A, float eta, const f
 /* a = tanh(5 tanh(m/5) + (softplus(s)+0.1) * eps)   (dreamer.py:197-200 with tanh_normal) */
 int pd_tanh_normal_sample(pd_handle* h, long rows, int A, const float* out, long ldo,
                           const float* eps, float* action, long lda, void* stream);
+/* normal_tanh policy (functions.py:59-66 with min_std 0.01, max_std 1; a2c.py:119-130 reinforce): out[rows,2A] = (m, s)
+ * raw, mu = tanh(m), sd = sigmoid(s) + 0.01, policy Independent(Normal(mu, sd), 1) with no transform on the action.
+ * sums[2] (double) += {sum (-log_prob(a) agae - eta entropy) w, sum entropy} with the Normal's entropy, added in a
+ * fixed order (bit-identical run to run); dout[rows,2A] = d mean(.)/d out.
+ * rows >= 0, A >= 1, ldo >= 2A, lddo >= 2A, lda >= A, otherwise PD_ERR_ARG before any launch; rows = 0 launches nothing. */
+int pd_actor_loss_normal_tanh(pd_handle* h, long rows, int A, float eta, const float* out, long ldo,
+                              const float* actions, long lda, const float* agae, const float* weight,
+                              float* dout, long lddo, double* sums, void* stream);
+/* a = tanh(m) + (sigmoid(s) + 0.01) * eps, unbounded   (dreamer.py:196-200 with normal_tanh: Normal.sample()).
+ * rows >= 0, A >= 1, ldo >= 2A, lda >= A, otherwise PD_ERR_ARG before any launch; rows = 0 launches nothing. */
+int pd_normal_tanh_sample(pd_handle* h, long rows, int A, const float* out, long ldo,
+                          const float* eps, float* action, long lda, void* stream);
 
 /* ---- replay preprocessing on the device (pydreamer/preprocessing.py:91-188; SURVEY.md §8f N3) ------------ */
 /* uint8 image (NB,H,W,C) -> fp32 (NB,C,H,W) = x/255 - 0.5 (preprocessing.py:21-29): the batch crosses PCIe as bytes. */

@@ -137,6 +137,18 @@ PRESETS = {
     "tiny_gru3_odd": (("atari",), dict(deter_dim=66, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4, action_dim=5,
                                        batch_size=3, batch_length=4, imag_horizon=3, gru_layers=3)),
     "atari_gru2": (("atari",), dict(deter_dim=2048, batch_size=50, batch_length=50, gru_layers=2)),
+    # the normal_tanh actor (Normal(tanh(m), sigmoid(s) + 0.01), actions not bounded): tiny DMC shapes, with three importance
+    # samples, without an image; then the DMC benchmark shape
+    "tiny_dmc_normaltanh": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                           action_dim=3, batch_size=3, batch_length=4, imag_horizon=3,
+                                           actor_grad="reinforce", actor_dist="normal_tanh")),
+    "tiny_dmc_normaltanh_iwae3": (("dmc",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, cnn_depth=4,
+                                                 action_dim=3, batch_size=3, batch_length=4, imag_horizon=3, iwae_samples=3,
+                                                 actor_grad="reinforce", actor_dist="normal_tanh")),
+    "tiny_vector_normaltanh": (("vectorenv",), dict(deter_dim=64, stoch_dim=4, stoch_discrete=8, hidden_dim=40, action_dim=3,
+                                                    batch_size=3, batch_length=4, imag_horizon=3, actor_dist="normal_tanh")),
+    "dmc_normaltanh": (("dmc",), dict(deter_dim=1024, batch_size=50, batch_length=50, actor_grad="reinforce",
+                                      actor_dist="normal_tanh")),
 }
 
 

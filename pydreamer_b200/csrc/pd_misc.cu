@@ -423,11 +423,16 @@ actor_loss_onehot_kernel(long rows, int A, float eta, const float* __restrict__ 
     sums_flush<2>(x, ws, ticket, sums);
 }
 
-__global__ void actor_loss_tanh_normal_kernel(long rows, int A, float eta, const float* __restrict__ out, long ldo,
-                                              const float* __restrict__ actions, long lda,
-                                              const float* __restrict__ agae, const float* __restrict__ weight,
-                                              float* __restrict__ dout, long lddo, double* sums, double* ws,
-                                              unsigned* ticket) {
+// The two Gaussian policies on out[rows, 2A] = (m, s) raw.  NT = false: tanh_normal (functions.py:69-78), the base
+// Normal(5 tanh(m/5), softplus(s) + 0.1) under a TanhTransform, log_prob through atanh of the clamped action, entropy of
+// the base distribution.  NT = true: normal_tanh (functions.py:59-66, min_std 0.01, max_std 1), Normal(tanh(m),
+// sigmoid(s) + 0.01) with no transform, so the action is unbounded and the entropy is the Normal's own.
+template <bool NT>
+__global__ void actor_loss_gaussian_kernel(long rows, int A, float eta, const float* __restrict__ out, long ldo,
+                                           const float* __restrict__ actions, long lda,
+                                           const float* __restrict__ agae, const float* __restrict__ weight,
+                                           float* __restrict__ dout, long lddo, double* sums, double* ws,
+                                           unsigned* ticket) {
     __shared__ double shd[2][8];
     const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
     double s_loss = 0, s_ent = 0;
@@ -437,21 +442,33 @@ __global__ void actor_loss_tanh_normal_kernel(long rows, int A, float eta, const
         const float eps = 1.1920928955078125e-07f;
         for (int i = 0; i < A; ++i) {
             float m_ = out[row * ldo + i], s_ = out[row * ldo + A + i];
-            float th = tanhf(m_ / 5.f);
-            float mu = 5.f * th;
-            float sd = pd_softplus(s_) + 0.1f;
-            float y = fminf(fmaxf(actions[row * lda + i], -1.f + eps), 1.f - eps);
-            float x = atanhf(y);
-            float zc = (x - mu) / sd;
-            // Normal.log_prob - TanhTransform.log_abs_det_jacobian
-            float lpn = -0.5f * zc * zc - logf(sd) - 0.9189385332046727f;
-            float ladj = 2.f * (0.6931471805599453f - x - pd_softplus(-2.f * x));
-            lp += lpn - ladj;
-            ent += 0.5f + 0.9189385332046727f + logf(sd);
-            float dlp_dmu = zc / sd;
-            float dlp_dsd = (zc * zc - 1.f) / sd;
-            dout[row * lddo + i] = w * inv * (-ag * dlp_dmu) * (1.f - th * th);
-            dout[row * lddo + A + i] = w * inv * (-ag * dlp_dsd - eta / sd) * pd_sigmoid(s_);
+            if constexpr (NT) {
+                float mu = tanhf(m_);
+                float sg = pd_sigmoid(s_);
+                float sd = sg + 0.01f;
+                float zc = (actions[row * lda + i] - mu) / sd;
+                float lsd = logf(sd);
+                lp += -0.5f * zc * zc - lsd - 0.9189385332046727f;
+                ent += 0.5f + 0.9189385332046727f + lsd;
+                dout[row * lddo + i] = w * inv * (-ag * (zc / sd)) * (1.f - mu * mu);
+                dout[row * lddo + A + i] = w * inv * (-ag * ((zc * zc - 1.f) / sd) - eta / sd) * (sg * (1.f - sg));
+            } else {
+                float th = tanhf(m_ / 5.f);
+                float mu = 5.f * th;
+                float sd = pd_softplus(s_) + 0.1f;
+                float y = fminf(fmaxf(actions[row * lda + i], -1.f + eps), 1.f - eps);
+                float x = atanhf(y);
+                float zc = (x - mu) / sd;
+                // Normal.log_prob - TanhTransform.log_abs_det_jacobian
+                float lpn = -0.5f * zc * zc - logf(sd) - 0.9189385332046727f;
+                float ladj = 2.f * (0.6931471805599453f - x - pd_softplus(-2.f * x));
+                lp += lpn - ladj;
+                ent += 0.5f + 0.9189385332046727f + logf(sd);
+                float dlp_dmu = zc / sd;
+                float dlp_dsd = (zc * zc - 1.f) / sd;
+                dout[row * lddo + i] = w * inv * (-ag * dlp_dmu) * (1.f - th * th);
+                dout[row * lddo + A + i] = w * inv * (-ag * dlp_dsd - eta / sd) * pd_sigmoid(s_);
+            }
         }
         s_loss = (double)((-lp * ag - eta * ent) * w);
         s_ent = ent;
@@ -469,13 +486,19 @@ __global__ void actor_loss_tanh_normal_kernel(long rows, int A, float eta, const
     sums_flush<2>(x, ws, ticket, sums);
 }
 
-__global__ void tanh_normal_sample_kernel(long rows, int A, const float* __restrict__ out, long ldo,
-                                          const float* __restrict__ eps, float* __restrict__ action, long lda) {
+template <bool NT>
+__global__ void gaussian_sample_kernel(long rows, int A, const float* __restrict__ out, long ldo,
+                                       const float* __restrict__ eps, float* __restrict__ action, long lda) {
     GRID_STRIDE(i, rows * A) {
         long r = i / A; int c = (int)(i % A);
-        float mu = 5.f * tanhf(out[r * ldo + c] / 5.f);
-        float sd = pd_softplus(out[r * ldo + A + c]) + 0.1f;
-        action[r * lda + c] = tanhf(mu + sd * eps[i]);
+        if constexpr (NT) {
+            float sd = pd_sigmoid(out[r * ldo + A + c]) + 0.01f;
+            action[r * lda + c] = tanhf(out[r * ldo + c]) + sd * eps[i];
+        } else {
+            float mu = 5.f * tanhf(out[r * ldo + c] / 5.f);
+            float sd = pd_softplus(out[r * ldo + A + c]) + 0.1f;
+            action[r * lda + c] = tanhf(mu + sd * eps[i]);
+        }
     }
 }
 
@@ -704,15 +727,44 @@ int pd_actor_loss_tanh_normal(pd_handle* h, long rows, int A, float eta, const f
     unsigned* tk;
     int rc = pd_scratch(h, S(stream), 2L * grid * 2, 1, &ws, &tk);          // grid x 2 doubles
     if (rc) return rc;
-    actor_loss_tanh_normal_kernel<<<grid, 256, 0, S(stream)>>>(rows, A, eta, out, ldo, actions, lda, agae, weight, dout, lddo, sums,
-                                                               (double*)ws, tk);
+    actor_loss_gaussian_kernel<false><<<grid, 256, 0, S(stream)>>>(rows, A, eta, out, ldo, actions, lda, agae, weight, dout,
+                                                                   lddo, sums, (double*)ws, tk);
     PD_CHECK_LAUNCH(h, "actor_loss_tanh_normal");
     return PD_OK;
 }
 int pd_tanh_normal_sample(pd_handle* h, long rows, int A, const float* out, long ldo, const float* eps, float* action,
                           long lda, void* stream) {
-    tanh_normal_sample_kernel<<<grid_for(rows * A, 256, h->num_sms), 256, 0, S(stream)>>>(rows, A, out, ldo, eps, action, lda);
+    gaussian_sample_kernel<false><<<grid_for(rows * A, 256, h->num_sms), 256, 0, S(stream)>>>(rows, A, out, ldo, eps, action,
+                                                                                              lda);
     PD_CHECK_LAUNCH(h, "tanh_normal_sample");
+    return PD_OK;
+}
+int pd_actor_loss_normal_tanh(pd_handle* h, long rows, int A, float eta, const float* out, long ldo,
+                              const float* actions, long lda, const float* agae, const float* weight, float* dout,
+                              long lddo, double* sums, void* stream) {
+    PD_REQUIRE(h, rows >= 0 && A >= 1 && ldo >= 2L * A && lda >= A && lddo >= 2L * A,
+               "pd_actor_loss_normal_tanh: rows=%ld (>= 0), A=%d (>= 1), ldo=%ld / lddo=%ld (>= 2A), lda=%ld (>= A) "
+               "unsupported", rows, A, ldo, lddo, lda);
+    if (rows == 0) return PD_OK;
+    const int grid = pd_cdiv(rows, 256);
+    float* ws;
+    unsigned* tk;
+    int rc = pd_scratch(h, S(stream), 2L * grid * 2, 1, &ws, &tk);          // grid x 2 doubles
+    if (rc) return rc;
+    actor_loss_gaussian_kernel<true><<<grid, 256, 0, S(stream)>>>(rows, A, eta, out, ldo, actions, lda, agae, weight, dout,
+                                                                  lddo, sums, (double*)ws, tk);
+    PD_CHECK_LAUNCH(h, "actor_loss_normal_tanh");
+    return PD_OK;
+}
+int pd_normal_tanh_sample(pd_handle* h, long rows, int A, const float* out, long ldo, const float* eps, float* action,
+                          long lda, void* stream) {
+    PD_REQUIRE(h, rows >= 0 && A >= 1 && ldo >= 2L * A && lda >= A,
+               "pd_normal_tanh_sample: rows=%ld (>= 0), A=%d (>= 1), ldo=%ld (>= 2A), lda=%ld (>= A) unsupported",
+               rows, A, ldo, lda);
+    if (rows == 0) return PD_OK;
+    gaussian_sample_kernel<true><<<grid_for(rows * A, 256, h->num_sms), 256, 0, S(stream)>>>(rows, A, out, ldo, eps, action,
+                                                                                             lda);
+    PD_CHECK_LAUNCH(h, "normal_tanh_sample");
     return PD_OK;
 }
 int pd_sumsq(pd_handle* h, const float* x, long n, float* out, float* ws, void* stream) {

@@ -469,7 +469,7 @@ class Dreamer(nn.Module):
             raise NotImplementedError("probe heads are research probes outside the hot path (SURVEY.md §2 row 9)")
         if conf.probe_gradients:
             raise NotImplementedError("probe_gradients is for the baselines (SURVEY.md §2 row 10)")
-        if conf.actor_dist not in ("onehot", "tanh_normal"):
+        if conf.actor_dist not in ("onehot", "tanh_normal", "normal_tanh"):
             raise NotImplementedError(f"actor_dist={conf.actor_dist}")
         if conf.actor_grad != "reinforce":
             raise NotImplementedError("actor_grad=dynamics asserts upstream at a2c.py:131 (SURVEY.md §0.5); "
@@ -711,12 +711,16 @@ class Dreamer(nn.Module):
         y = alog.view(1, B, d.Aout).clone()
         if self.conf.actor_dist == "onehot":
             dist = D.OneHotCategorical(logits=y)
-        else:                                                          # functions.py:69-78
+        elif self.conf.actor_dist == "tanh_normal":                    # functions.py:69-78
             mean = 5 * torch.tanh(y[..., :d.A] / 5)
             std = torch.nn.functional.softplus(y[..., d.A:]) + 0.1
             normal = D.independent.Independent(D.normal.Normal(mean, std), 1)
             dist = D.TransformedDistribution(normal, [D.TanhTransform()])
             dist.entropy = normal.entropy
+        else:                                                          # normal_tanh, functions.py:59-66
+            mean = torch.tanh(y[..., :d.A])
+            std = torch.sigmoid(y[..., d.A:]) + 0.01
+            dist = D.independent.Independent(D.normal.Normal(mean, std), 1)
         return dist, out_state, dict(policy_value=val.mean())
 
     # ------------------------------------------------------------------ workspace
@@ -892,7 +896,7 @@ class Dreamer(nn.Module):
     # ------------------------------------------------------------------ noise
     def _draw_noise(self, T, BI, N, H, image_pred=False, dream_log=False, B=0):
         """Exp(1) noise for the categorical samples in the reference's consumption order (SURVEY.md App. D);
-        Gaussian noise for the tanh_normal actor."""
+        Gaussian noise for the tanh_normal and normal_tanh actors."""
         d, dev = self.d, self._arena.device
         post = self._buf("noise.post", T, BI, d.Z).exponential_()
         actor = self._buf("noise.actor", H, N, d.A)
@@ -1790,8 +1794,10 @@ class Dreamer(nn.Module):
             onehot = conf.actor_dist == "onehot"
             if onehot:
                 ops.cat_sample(dr.alog[i], noise_actor[i], 1, d.A, dr.actions[i], idx=aidx)
-            else:
+            elif conf.actor_dist == "tanh_normal":
                 ops.tanh_normal_sample(dr.alog[i], noise_actor[i], dr.actions[i])
+            else:
+                ops.normal_tanh_sample(dr.alog[i], noise_actor[i], dr.actions[i])
             if onehot and d.Hd % 4 == 0:
                 ops.gather_rows(aidx, self._waT, aa)                 # a_mlp(one-hot) = one row of a_mlp^T
             else:
@@ -1846,8 +1852,10 @@ class Dreamer(nn.Module):
         dal = b("ac.dalog", H * N, d.Ap)[:, :d.Aout]
         if conf.actor_dist == "onehot":
             ops.actor_loss_onehot(conf.entropy, alog, actions, agae, weight, dal, sums[5:7])
-        else:
+        elif conf.actor_dist == "tanh_normal":
             ops.actor_loss_tanh_normal(conf.entropy, alog, actions, agae, weight, dal, sums[5:7])
+        else:
+            ops.actor_loss_normal_tanh(conf.entropy, alog, actions, agae, weight, dal, sums[5:7])
         if want_grad:
             fH = fall[:H * N]
             self._mlp_bwd(cp, fH, dv, critic)

@@ -421,6 +421,17 @@ class NativeOps:
         self._ck(self.lib.pd_tanh_normal_sample(self.h, rows, A, _ptr(out), _ld(out), _ptr(eps), _ptr(action),
                                                 _ld(action), self._s()), "pd_tanh_normal_sample")
 
+    def actor_loss_normal_tanh(self, eta, out, actions, agae, weight, dout, sums):
+        rows, A = actions.shape
+        self._ck(self.lib.pd_actor_loss_normal_tanh(self.h, rows, A, float(eta), _ptr(out), _ld(out), _ptr(actions),
+                                                    _ld(actions), _ptr(agae), _ptr(weight), _ptr(dout), _ld(dout),
+                                                    _ptr(sums), self._s()), "pd_actor_loss_normal_tanh")
+
+    def normal_tanh_sample(self, out, eps, action):
+        rows, A = action.shape
+        self._ck(self.lib.pd_normal_tanh_sample(self.h, rows, A, _ptr(out), _ld(out), _ptr(eps), _ptr(action),
+                                                _ld(action), self._s()), "pd_normal_tanh_sample")
+
     # ------------------------------------------------------------------ preprocessing
     def image_u8_to_f32(self, src, dst):
         NB = src.numel() // (src.shape[-1] * src.shape[-2] * src.shape[-3])
